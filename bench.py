@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- VO frames/s of the DF-VO tracking hot path on B200 (BASELINE.json metric).
+"""bench.py -- VO frames/s of the DF-VO tracking hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|torch_gpu]
-                    [--config vo|corr64|ransac10k|pairs64|parity] [--no-extras]
+                    [--config vo|corr64|ransac10k|pairs64|parity] [--no-extras] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Default workload (`--config vo`, BASELINE.json configs[1]): KITTI-odometry-shaped stream of 376x1241 RGB frames, full hybrid
@@ -26,10 +26,14 @@ all with identical poses); `e2e.latency_ms` is the time from handing a frame to 
 Output: ONE JSON line (rank 0).  `value` = frames/s with frames already in HBM; `e2e` = the same metric through the public API
 (pinned host uint8 frames -> pose on the host) with H2D/D2H inside the timed region; `e2e_libs` = through the reference-API
 mirror (`libs.deep_models.DeepModel.forward_depth/forward_flow`, `KeypointSampler`, `EssTracker`, `PnpTracker`) the way
-libs/dfvo.py calls it; `roofline` = the tcgen05 convolution kernels against the measured bf16 peak (per-launch CUDA events on
+libs/dfvo.py calls it; `roofline` = the wgmma convolution kernels against the data-sheet bf16 peak (per-launch CUDA events on
 an in-order stream); `cpu_baseline` = the CPU oracle port of the same frame timed on this box's cores; `precision_modes` = the
 same pipeline in tf32 / fp32 mode; `gpu_library_baseline` = the reference graph through torch/cuDNN on the same GPU;
 `extra_configs` = BASELINE configs[2] (correlation + consistency, HBM roofline) and configs[3] (RANSAC scoring, FP64 roofline).
+
+--dump-outputs DIR (default config): after the timed steps, writes what the timed path returned in its last step, the 4x4 pose
+`FramePipeline.step` handed back, as DIR/pose.npy (float64).  Inputs and weights are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import ctypes
@@ -55,7 +59,7 @@ N_DISTINCT = 8                     # distinct synthetic frames cycled through th
 FRAME_MODES = ["normal"] * N_DISTINCT
 FRAME_MODES[5] = "still"           # one PnP-fallback frame per cycle (GRIC prefers the homography)
 FRAME_OUTLIERS = [0.0, 0.3, 0.6, 0.0, 0.3, 0.0, 0.6, 0.0]      # SURVEY 8d sweep, cycled
-FP64_PEAK_TFLOPS = 40.0            # nominal B200 FP64 FMA peak (SURVEY 8d; no measured figure in MEASURED_PEAKS.json)
+FP64_PEAK_TFLOPS = 34.0            # H100 SXM data-sheet FP64 peak without tensor cores (the RANSAC kernels use FMA units)
 
 
 def parse():
@@ -67,6 +71,8 @@ def parse():
     ap.add_argument("--config", default="vo", choices=["vo", "corr64", "ransac10k", "pairs64", "parity"])
     ap.add_argument("--cpu-frames", type=int, default=3, help="frames of the CPU baseline sample")
     ap.add_argument("--no-extras", action="store_true", help="skip precision modes / library baseline / extra configs / e2e_libs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the pose the last timed step returned to DIR/pose.npy (float64)")
     ap.add_argument("--diag-no-track", action="store_true",
                     help="DIAGNOSTIC, not a bench value: replace the tracker by an identity pose to see the networks-only ceiling of the pipeline")
     return ap.parse_args()
@@ -213,7 +219,7 @@ def run_reference(args):
     line = dict(impl="reference", metric=METRIC, value=base["value"], unit="frames/s", n_gpus=args.gpus, steps=n, warmup=1,
                 ms_per_step=1e3 / base["value"], higher_is_better=True, scaling="weak", vs_baseline=None, dtype="f32",
                 data="synthetic", config=dict(workload=WORKLOAD, note="reference's CPU path = oracle port (the reference is pure "
-                "Python + torch/cv2/sklearn; /root/reference does not travel to the GPU box)"),
+                "Python + torch/cv2/sklearn)"),
                 cpu_baseline=base, e2e=dict(value=base["value"], unit="frames/s", h2d_bytes_per_step=0, d2h_bytes_per_step=0))
     print(json.dumps(line))
 
@@ -223,8 +229,7 @@ def run_reference(args):
 # ------------------------------------------------------------------------------------------------
 def torch_gpu_baseline(frames, iters=8):
     """oracle/nets.py (the functional restatement of the reference modules) executed by torch on cuda: cuDNN convolutions,
-    the correlation as 49 shifted multiply-reduce torch ops (the reference's own cupy kernel needs cupy; its kernel text lives
-    under /root/reference, which does not travel).  Three settings: strict fp32, TF32 (torch's default for cuDNN convs), and
+    the correlation as 49 shifted multiply-reduce torch ops (the reference's own cupy kernel needs cupy).  Three settings: strict fp32, TF32 (torch's default for cuDNN convs), and
     bf16 autocast + channels_last.  A BASELINE measurement: nothing of the product runs here."""
     import torch
     import torch.nn.functional as F
@@ -325,12 +330,12 @@ def bench_corr64(rt, pairs=64, iters=5):
     """Times `dfvo_correlation_nhwc_bf16` (the kernel of the product path, on its own NHWC bf16 layout) for B = 2*pairs maps
     at each pyramid level, and `dfvo_fb_consistency` for `pairs` 376x1241 flow pairs.  Algorithmic bytes (SURVEY 8d, bytes
     *touched*, bf16 = half the fp32 figures): first operand at the sampled pixels + the (7s)^2-window union of the second
-    operand (= the whole map) + the 49-channel output; consistency 20 B / pixel.  Inputs exceed the 126 MB L2 at levels 2-4;
+    operand (= the whole map) + the 49-channel output; consistency 20 B / pixel.  Inputs exceed the 50 MB L2 at levels 2-4;
     the small levels are timed L2-warm, as they run in the network."""
     import torch
     lib = rt.lib
     B = 2 * pairs
-    hbm = float(peaks().get("hbm_gbs", 6650.0))
+    hbm = float(peaks().get("hbm_gbs", 3350.0))
     rows, tot_bytes, tot_ms = [], 0.0, 0.0
     ev = lambda: torch.cuda.Event(enable_timing=True)
     for (L, C, h, w, s) in CORR_LEVELS:
@@ -376,7 +381,7 @@ def bench_corr64(rt, pairs=64, iters=5):
     return dict(workload="BASELINE configs[2]: %d pairs, correlation at the five level shapes (bf16 NHWC) + fwd-bwd consistency" % pairs,
                 levels=rows, fb_consistency=fbrow, total_ms=tot_ms, total_algorithmic_gb=tot_bytes / 1e9, gbs=tot_bytes / tot_ms / 1e6,
                 roofline=dict(bound="hbm", achieved=tot_bytes / tot_ms / 1e6, peak=hbm, unit="GB/s", frac=tot_bytes / tot_ms / 1e6 / hbm,
-                              peak_source="MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks() else "fallback 6.65 TB/s"))
+                              peak_source="MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks() else "H100 SXM data sheet 3.35 TB/s (not a measured figure)"))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -421,7 +426,7 @@ def bench_ransac10k(rt, iters=10):
     out = dict(workload="BASELINE configs[3]: Sampson scoring of %d hypotheses x %d correspondences, FP64" % (M, N), scoring_ms=ms,
                algorithmic_gflop=flop / 1e9, evaluations_per_s=M * N / ms * 1e3,
                roofline=dict(bound="fp64", achieved=flop / ms / 1e9, peak=FP64_PEAK_TFLOPS, unit="TFLOP/s", frac=flop / ms / 1e9 / FP64_PEAK_TFLOPS,
-                             peak_source="nominal B200 FP64 FMA peak (SURVEY 8d); FLOPs = 33 per (model, correspondence)"),
+                             peak_source="H100 SXM data-sheet FP64 peak without tensor cores, 34 TFLOP/s; FLOPs = 33 per (model, correspondence)"),
                inliers_max=int(cnt.numpy().max()))
     # the full replayed RANSAC (5 repeats + GRIC + homography vote + recoverPose) per outlier fraction
     eng = tracking.Engine(H, W, rt)
@@ -498,7 +503,7 @@ def run_pairs64(args):
                 dtype="bf16 tensor-core convs (fp32 accumulate)", data="synthetic frames + seeded random-init weights",
                 config=dict(workload="64 independent 376x1241 image pairs, contiguous block of 64/N pairs per GPU, one batched forward per step; NCCL weight "
                             "broadcast + one all_gather of the per-pair consistency statistics", pairs_per_gpu=sh.count,
-                            l2="activation working set of one rank (>0.5 GB per pair) exceeds the 126 MB L2"),
+                            l2="activation working set of one rank (>0.5 GB per pair) exceeds the 50 MB L2"),
                 gpu_launches=int(launches), pair_stats=dict(n=len(all_stats), mean_flow_diff_first=float(all_stats[0][0]), mean_flow_diff_last=float(all_stats[-1][0])))
     print(json.dumps(line))
     if world > 1:
@@ -619,8 +624,8 @@ def run_b200(args):
 
     K, frames, analytic = make_inputs(rank)
     overlap = os.environ.get("DFVO_OVERLAP", "1") != "0"
-    # network engines in flight.  Measured (profiles/r02_pipeline_modes.json): 3 engines + pipelined tracker 446 fps at 11.2 ms latency,
-    # 2 engines + tracker read in the same step 421 fps at 7.1 ms (reported as e2e.low_latency), 1 engine 362 fps
+    # network engines in flight: 3 engines + pipelined tracker by default; 2 engines with the tracker read in the same step are
+    # reported as e2e.low_latency
     inflight = int(os.environ.get("DFVO_INFLIGHT", "3")) if overlap else 1
 
     # device-resident copies of everything a step consumes
@@ -694,6 +699,8 @@ def run_b200(args):
             slot = fid % N_DISTINCT
             submit[fid] = time.perf_counter()
             pose = pipe.step(d_frames[slot] if resident else pinned[slot])
+            if pose is not None:
+                state["last_pose"] = pose
             if pose is not None and (fid - lag) in submit:
                 lat.append(time.perf_counter() - submit[fid - lag])
         if pipe.overlap:                  # the closing event waits for all of the pipeline's streams
@@ -726,7 +733,9 @@ def run_b200(args):
     clocks = Clocks(local_rank)
     if rank == 0:
         clocks.start()
+    state.pop("last_pose", None)
     ms, launches, _ = timed(pipe, args.steps, True, clocks if rank == 0 else None)
+    last_pose = state.pop("last_pose", None)
     clk = clocks.stop() if rank == 0 else None
     ms_e2e, _, lat_e2e = timed(pipe, args.steps, False)
     h2d, d2h = state["h2d"] / args.steps, state["d2h"] / args.steps
@@ -763,7 +772,7 @@ def run_b200(args):
                        what="FramePipeline(overlap=True, inflight=2, pipelined=False): two network engines, step(t) returns the pose of frame t-2")
         del p2
 
-    # ---------------------------------------------------------------- roofline of the dominant kernels (tcgen05 convs)
+    # ---------------------------------------------------------------- roofline of the dominant kernels (wgmma convs)
     # CUDA-event timing of every launch over a few steps, on an in-order single-stream pipeline sharing the built networks (in
     # the two-stream pipeline the tracker's and the depth network's kernels run beside the convolutions, which would be charged
     # to whichever launch they overlap)
@@ -820,16 +829,16 @@ def run_b200(args):
 
     if rank != 0:
         return
+    if args.dump_outputs:
+        assert last_pose is not None, "no timed step returned a pose (raise --steps)"
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "pose.npy"), np.asarray(last_pose, dtype=np.float64))
     pk = peaks()
-    peak_tf = float(pk.get("bf16_tflops_sustained", 1400.0))
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in pk else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
+    peak_tf = float(pk.get("bf16_tflops_sustained", 989.0))
+    peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in pk else
+                "H100 SXM data sheet, dense bf16 989 TFLOP/s at up to 700 W (not a measured figure)")
     achieved = (tc_fl.value / 1e12) / (tc_ms.value / 1e3) if tc_ms.value > 0 else 0.0
-    traffic, traffic_src = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "conv_tc_traffic.json")))
-        traffic, traffic_src = tj["dram_bytes_per_frame"], "ncu dram__bytes_read.sum + dram__bytes_write.sum of the conv launches of one frame, " + tj.get("source", "profiles/ (round 1)")
-    except Exception:
-        pass
+    traffic, traffic_src = None, "not measured"
     if args.cpu_frames > 0 and world == 1:
         base, cpu_poses = cpu_baseline(args.cpu_frames, K, frames, analytic)
     else:
@@ -845,7 +854,7 @@ def run_b200(args):
                     streams=("%d network engine(s) on their own streams, tracker %d frame(s) behind (%s); K steps = K frames inferred and K tracked"
                              % (inflight, pipe.lag, "its kernels enqueued in one step, its result read in the next" if pipe.pipelined else
                                 "enqueued and read in the same step")) if overlap else "1 (in order)",
-                    l2="per-frame activation working set (>1 GB written/read per frame) exceeds the 126 MB L2; no explicit flush",
+                    l2="per-frame activation working set (>1 GB written/read per frame) exceeds the 50 MB L2; no explicit flush",
                     frame_cycle=dict(modes=FRAME_MODES, outlier_fractions=FRAME_OUTLIERS), tracker_ms_by_branch_and_outliers=tracker_ms,
                     precision_modes=prec_modes),
         clocks=clk,
@@ -854,7 +863,7 @@ def run_b200(args):
                  in_order=inorder, low_latency=low_lat),
         e2e_libs=e2e_libs,
         gpu_launches=int(launches),
-        roofline=dict(kernel="k_conv_halo / k_conv_tc (tcgen05 implicit-GEMM conv, %d launches/frame)" % (tc_n.value // prof_steps), bound="tensor",
+        roofline=dict(kernel="k_conv_halo / k_conv_tc (wgmma implicit-GEMM conv, %d launches/frame)" % (tc_n.value // prof_steps), bound="tensor",
                       achieved=achieved, peak=peak_tf, unit="TFLOP/s", frac=achieved / peak_tf if peak_tf else None, traffic=traffic,
                       traffic_source=traffic_src, peak_source=peak_src, algorithmic_gflop_per_frame=tc_fl.value / prof_steps / 1e9,
                       kernel_ms_per_frame=tc_ms.value / prof_steps,

@@ -5,7 +5,7 @@ shards over *sequences*: rank r owns sequences r, r+world, ... and runs them wit
 received once at start-up.  That broadcast is the only collective; there is no data-path exchange, hence no
 fused compute+collective kernel to write (DESIGN.md section 7).  Timing is the max over ranks.
 
-Works on any torch.distributed backend: NCCL on the GPU box, gloo in the CPU test-suite
+Works on any torch.distributed backend: NCCL on GPUs, gloo in the CPU test-suite
 (tests/test_multi_gloo.py).
 """
 import numpy as np

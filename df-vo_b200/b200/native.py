@@ -184,7 +184,7 @@ def load(build_if_needed=True):
         m.build()
     lib = Lib(LIB_PATH)
     if lib.dfvo_is_device_build() != 1:
-        raise DfvoError("%s is not a device (nvcc, sm_100a) build" % LIB_PATH)
+        raise DfvoError("%s is not a device (nvcc, sm_90a) build" % LIB_PATH)
     _lib = lib
     return lib
 
@@ -192,4 +192,4 @@ def load(build_if_needed=True):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise DfvoError("dfvo_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise DfvoError("dfvo_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")

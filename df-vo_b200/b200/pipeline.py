@@ -1,7 +1,7 @@
 """Device-resident DF-VO frame pipeline: uint8 frame in, 4x4 pose out.
 
 The same per-frame algorithm as the reference driver's ``deep_model_inference`` + ``tracking``
-(dfvo.py:121-262,299-345, hybrid tracking, default configuration) but organised for the B200:
+(dfvo.py:121-262,299-345, hybrid tracking, default configuration) but organised for the GPU:
 everything from the uploaded frame to the keypoints / RANSAC scores / triangulated depths stays in HBM;
 the host only draws the RNG-dependent permutations, takes the small decisions the reference takes on the
 host (GRIC vote, cheirality threshold, sentinels) and chains the pose.  Per frame the host receives a few
@@ -74,8 +74,7 @@ class FramePipeline:
         tracker_thread=True (overlap mode only): the tracker runs on its own host thread (one frame at a time, in frame order, so
         the RNG stream and the poses are unchanged).  ``step(img)`` enqueues the networks of ``img``, hands the frame to the tracker
         thread and then waits for the pose of frame t-inflight, which that thread has been working on meanwhile: the host work
-        of enqueueing a frame (~0.4 ms) and the tracker's device waits (1.6-3.4 ms per frame) overlap instead of adding up.
-        Measured on B200: the networks alone sustain 1.9 ms per frame with two engines; the single-thread pipeline 2.6."""
+        of enqueueing a frame and the tracker's device waits overlap instead of adding up."""
         self.cfg = cfg or cfg_mod.default_cfg(height, width)
         self.K = [float(v) for v in K]
         self.H, self.W = height, width

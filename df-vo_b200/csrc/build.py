@@ -1,8 +1,8 @@
-"""Build libdfvo_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libdfvo_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python df-vo_b200/csrc/build.py [--force]
 
-The .so stays next to the sources (git-ignored, but it travels to the GPU box with gpurun).
+The .so stays next to the sources (git-ignored).
 """
 import hashlib
 import os
@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["capi.cu", "net_common.cu", "flow_ops.cu", "conv_direct.cu", "conv_tc.cu", "conv_halo.cu", "conv_chain.cu", "liteflownet.cu", "select.cu", "ransac.cu", "pnp.cu", "homog.cu", "depth_ops.cu", "monodepth2.cu", "geometry.cu", "corr_mma.cu"]
 NO_FMA = {"ransac.cu", "pnp.cu", "homog.cu"}
 OUT = os.path.join(HERE, "libdfvo_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 

@@ -174,7 +174,7 @@ static int stage_conv(const float* x, const HostTensor& w, const HostTensor* b, 
 extern "C" {
 
 const char* dfvo_last_error(void) { return dfvo::last_error(); }
-const char* dfvo_version(void) { return "dfvo_b200 0.1 (sm_100a)"; }
+const char* dfvo_version(void) { return "dfvo_b200 0.1 (sm_90a)"; }
 int dfvo_is_device_build(void) {
 #ifdef DFVO_HOSTSIM
   return 0;
@@ -330,7 +330,7 @@ int dfvo_conv2d(const float* x, const float* w_host, const float* bias_host, flo
   if (precision == DFVO_PREC_FP32)
     return stage_conv<float>(x, w, bias_host ? &b : nullptr, y, B, Cin, H, W, Cout, kh, kw, stride, pad_y, pad_x, reflect, act, (cudaStream_t)stream);
   DFVO_REQUIRE((stride == 1 || (stride == 2 && H % 2 == 0 && W % 2 == 0 && kh % 2 == 1 && pad_y == kh / 2 && pad_x == kw / 2)) && !reflect,
-               DFVO_EINVAL, "dfvo_conv2d: the tcgen05 path needs stride 1, or stride 2 on even sizes with 'same' padding; zero padding");
+               DFVO_EINVAL, "dfvo_conv2d: the tensor-core path needs stride 1, or stride 2 on even sizes with 'same' padding; zero padding");
   if (precision == DFVO_PREC_TF32)
     return stage_conv<float>(x, w, bias_host ? &b : nullptr, y, B, Cin, H, W, Cout, kh, kw, stride, pad_y, pad_x, reflect, act, (cudaStream_t)stream, true);
   return stage_conv<bf16>(x, w, bias_host ? &b : nullptr, y, B, Cin, H, W, Cout, kh, kw, stride, pad_y, pad_x, reflect, act, (cudaStream_t)stream);

@@ -2,17 +2,15 @@
 // Subpixel / Regularization main stacks, lite_flow_net.py:98-240) in ONE persistent cooperative launch, with a grid-wide barrier
 // between layers instead of a kernel boundary.
 //
-// Why: the coarse pyramid levels are chains of tiny layers (11x38 ... 44x152 pixels, 1 tile per CTA).  In-kernel phase stamps
-// (profiles/r02_halo_phase_stamps.txt) show such a layer needs ~4.4 us on the SM -- 1.0 us TMA latency, ~2 us of MMAs, ~0.9 us
-// epilogue -- while a launch of its own costs 8-10 us of GPU time (grid launch, 200 KB shared-memory / TMEM set-up and tear-down,
-// completion + flush); 60-odd such launches per frame were ~0.8 ms of the 2.3 ms the convolutions take.  Inside a chain a layer
-// boundary is one release/acquire counter in global memory (~1.5 us) and the weight stream of the next layer is prefetched across
-// it (the B producer never waits for the barrier).
+// Why: the coarse pyramid levels are chains of tiny layers (11x38 ... 44x152 pixels, 1 tile per CTA) whose few microseconds of
+// work on the SM are small next to the fixed cost of a launch of their own (grid launch, ~200 KB shared-memory set-up, completion
+// and flush).  Inside a chain a layer boundary is one release/acquire counter in global memory, and the weight stream of the next
+// layer is prefetched across it (the B producer never waits for the barrier).
 //
-// Same tile machinery as conv_halo.cu (halo-resident A operand, shifted UMMA descriptors per tap, S sub-tiles share B, warp roles
-// A-producer / B-producer / MMA / 8 epilogue warps, double-buffered TMEM accumulators); the ring geometry (slot sizes, stage counts)
-// is fixed per chain, everything else (window, channels, block_n, activation, output) is per layer.
-// Memory-model notes: a layer's outputs are written with generic-proxy stores by the epilogue warps of all CTAs and read by the next
+// Same tile machinery as conv_halo.cu (halo-resident A operand, shifted wgmma descriptors per tap, S sub-tiles share B, warp roles
+// A-producer / B-producer / two consumer warpgroups: tc_ptx.cuh::halo_tile_mma + halo_tile_store); the ring geometry (slot sizes,
+// stage counts) is fixed per chain, everything else (window, channels, block_n, activation, output) is per layer.
+// Memory-model notes: a layer's outputs are written with generic-proxy stores by the consumer warps of all CTAs and read by the next
 // layer's TMA loads (async proxy) of other CTAs.  Writers: st.global, fence.proxy.async, __threadfence, then ONE red.release.gpu per CTA.
 // Reader (the A producer's elected lane): ld.acquire.gpu spin until all CTAs arrived, fence.proxy.async, then the TMA loads.
 // All CTAs must be co-resident: the launcher uses a cooperative launch with grid <= #SMs (1 CTA per SM by shared memory).
@@ -29,14 +27,14 @@
 namespace dfvo {
 
 #define CHAIN_MAXL 12
-#define CHAIN_THREADS 352
+#define CHAIN_THREADS 384
 #define CHAIN_TH 16
 
 struct ChainL {
   int N, H, W, tiles_x, tiles_y, n_blocks, ntiles;
   int nsrc, srcC[3];
   int kh, kw, dy0, dx0, HW, HH;
-  int block_n, acc_cols;
+  int block_n;
   int Cout, Cout_pad, act, out_f32, zero_pad_to;
   const float* bias;
   void* out; long long oN, oH, oW;
@@ -47,7 +45,7 @@ struct alignas(64) ChainArgs {
   CUtensorMap tmA[CHAIN_MAXL][3];
   CUtensorMap tmB[CHAIN_MAXL];
   ChainL L[CHAIN_MAXL];
-  int nlayers, a_stages, b_stages, a_stage_bytes, b_stage_bytes, tmem_cols, bias_cap, pad;
+  int nlayers, a_stages, b_stages, a_stage_bytes, b_stage_bytes, bias_cap, pad0, pad1;
   unsigned* bar;            // [nlayers] arrival counters, zeroed by the launcher
   unsigned* err;            // set if a barrier wait gave up (watchdog)
 };
@@ -65,6 +63,21 @@ __device__ __forceinline__ bool chain_wait(const unsigned* ctr, unsigned target)
   return false;
 }
 
+// the tiles of one layer for one consumer warpgroup (block_n is a template parameter of the wgmma shape)
+template <int S, int BN>
+__device__ __noinline__ void chain_layer(const ChainL& p, TcRing& ra, TcRing& rb, const TcEpi& ep, const float* bias_s, int wg, int wq,
+                                            int lane, bool leader) {
+  float acc[S][BN / 2];
+  for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+    halo_tile_mma<S, BN, 0>(acc, ra, rb, p.nsrc, p.srcC, 64, 2, p.kh, p.kw, p.HW, wg, leader);
+    int t = tile;
+    const int tx = t % p.tiles_x; t /= p.tiles_x;
+    const int ty = t % p.tiles_y; t /= p.tiles_y;
+    const int n = t % p.N; const int nb = t / p.N;
+    halo_tile_store<S, BN>(acc, ep, bias_s, nb * BN, n, tx * 8 * S, ty * CHAIN_TH, p.W, p.H, p.oN, p.oH, p.oW, p.rN, p.rH, p.rW, wg, wq, lane);
+  }
+}
+
 template <int S>
 __global__ void __launch_bounds__(CHAIN_THREADS, 1)
 k_conv_chain(const __grid_constant__ ChainArgs P) {
@@ -76,37 +89,22 @@ k_conv_chain(const __grid_constant__ ChainArgs P) {
   const uint32_t a_base = base;
   const uint32_t b_base = base + (uint32_t)P.a_stages * (uint32_t)P.a_stage_bytes;
   const uint32_t bar_base = b_base + (uint32_t)P.b_stages * (uint32_t)P.b_stage_bytes;
-  auto a_full = [&](int s) { return bar_base + 8u * (uint32_t)s; };
-  auto a_empty = [&](int s) { return bar_base + 8u * (uint32_t)(P.a_stages + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (uint32_t)(2 * P.a_stages + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (uint32_t)(2 * P.a_stages + P.b_stages + s); };
-  const int nbar0 = 2 * P.a_stages + 2 * P.b_stages;
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (uint32_t)(nbar0 + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (uint32_t)(nbar0 + 2 + a); };
-  uint8_t* after_bars = base_ptr + (bar_base - base) + 8u * (uint32_t)(nbar0 + 4);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(after_bars);
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 4);
+  TcRing ra{a_base, (uint32_t)P.a_stage_bytes, bar_base, bar_base + 8u * (uint32_t)P.a_stages, P.a_stages, 0, 0u};
+  TcRing rb{b_base, (uint32_t)P.b_stage_bytes, bar_base + 16u * (uint32_t)P.a_stages, bar_base + 16u * (uint32_t)P.a_stages + 8u * (uint32_t)P.b_stages,
+            P.b_stages, 0, 0u};
+  float* bias_s = reinterpret_cast<float*>(base_ptr + (bar_base - base) + 16u * (uint32_t)(P.a_stages + P.b_stages));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 0 && lane == 0) {
     for (int l = 0; l < P.nlayers; ++l) { prefetch_tmap(&P.tmA[l][0]); prefetch_tmap(&P.tmB[l]); }
-    for (int s = 0; s < P.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 1); }
-    for (int s = 0; s < P.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 8); }
+    for (int s = 0; s < P.a_stages; ++s) { mbar_init(ra.full0 + 8u * s, 1); mbar_init(ra.empty0 + 8u * s, 2); }
+    for (int s = 0; s < P.b_stages; ++s) { mbar_init(rb.full0 + 8u * s, 1); mbar_init(rb.empty0 + 8u * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)P.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================================== A producer ===================================================================
-    int stage = 0; uint32_t phase = 0;
     for (int l = 0; l < P.nlayers; ++l) {
       const ChainL& p = P.L[l];
       if (l > 0) {                                            // every CTA has written its part of layer l-1
@@ -126,20 +124,19 @@ k_conv_chain(const __grid_constant__ ChainArgs P) {
         for (int s = 0; s < p.nsrc; ++s) {
           const CUtensorMap* tm = &P.tmA[l][s];
           for (int c0 = 0; c0 < p.srcC[s]; c0 += 64) {
-            mbar_wait(a_empty(stage), phase ^ 1u);
+            mbar_wait(ra.empty(), ra.ph ^ 1u);
             if (elect_one()) {
-              mbar_expect_tx(a_full(stage), a_bytes);
-              tma_load_4d(a_base + (uint32_t)stage * (uint32_t)P.a_stage_bytes, tm, a_full(stage), c0, x0, y0, n);
+              mbar_expect_tx(ra.full(), a_bytes);
+              tma_load_4d(ra.slot(), tm, ra.full(), c0, x0, y0, n);
             }
             __syncwarp();
-            if (++stage == P.a_stages) { stage = 0; phase ^= 1u; }
+            ra.next();
           }
         }
       }
     }
   } else if (warp == 1) {
     // ===================================== B producer: weights are constants -- runs ahead across layer boundaries ========
-    int stage = 0; uint32_t phase = 0;
     for (int l = 0; l < P.nlayers; ++l) {
       const ChainL& p = P.L[l];
       const int ntaps = p.kh * p.kw;
@@ -150,169 +147,49 @@ k_conv_chain(const __grid_constant__ ChainArgs P) {
         for (int s = 0; s < p.nsrc; ++s) {
           for (int c0 = 0; c0 < p.srcC[s]; c0 += 64) {
             for (int tap = 0; tap < ntaps; ++tap) {
-              mbar_wait(b_empty(stage), phase ^ 1u);
+              mbar_wait(rb.empty(), rb.ph ^ 1u);
               if (elect_one()) {
-                mbar_expect_tx(b_full(stage), b_bytes);
-                tma_load_3d(b_base + (uint32_t)stage * (uint32_t)P.b_stage_bytes, &P.tmB[l], b_full(stage), kofs + c0, nb * p.block_n, tap);
+                mbar_expect_tx(rb.full(), b_bytes);
+                tma_load_3d(rb.slot(), &P.tmB[l], rb.full(), kofs + c0, nb * p.block_n, tap);
               }
               __syncwarp();
-              if (++stage == P.b_stages) { stage = 0; phase ^= 1u; }
+              rb.next();
             }
           }
           kofs += p.srcC[s];
         }
       }
     }
-  } else if (warp == 2) {
-    // ===================================== MMA issuer ====================================================================
-    const uint32_t b_hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-    const uint32_t b_lo_base = ((b_base >> 4) & 0x3FFFu) | (1u << 16), b_lo_step = (uint32_t)P.b_stage_bytes >> 4;
-    const uint32_t b_full0 = b_full(0), b_empty0 = b_empty(0);
-    const int a_stages = P.a_stages, b_stages = P.b_stages;
-    int astage = 0; uint32_t aphase = 0;
-    int bstage = 0; uint32_t bphase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
+  } else if (warp >= 4) {
+    // ============================ two consumer warpgroups: MMA + epilogue ================================================
+    const int ct = threadIdx.x - 128, wg = ct >> 7, wq = (ct >> 5) & 3;
+    const bool leader = (ct & 127) == 0;
     for (int l = 0; l < P.nlayers; ++l) {
       const ChainL& p = P.L[l];
-      const uint32_t idesc = tc_idesc(0, p.block_n);
-      const uint32_t a_hi = (((uint32_t)p.HW * 128u) >> 4) | (1u << 14) | (2u << 29);
-      const int kh = p.kh, kw = p.kw;
-      const uint32_t row_skip = (uint32_t)(p.HW - p.kw) * 8u;
-      const uint32_t bn = (uint32_t)p.block_n;
-      for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * p.acc_cols);
-        uint32_t fresh = 0;
-        for (int s = 0; s < p.nsrc; ++s) {
-          for (int c0 = 0; c0 < p.srcC[s]; c0 += 64) {
-            mbar_wait(a_full(astage), aphase);
-            tc_fence_after();
-            const uint32_t a_lo0 = (((a_base + (uint32_t)astage * (uint32_t)P.a_stage_bytes) >> 4) & 0x3FFFu) | (1u << 16);
-            const int rem = p.srcC[s] - c0;
-            const int nks = (rem >= 64 ? 64 : rem) >> 4;
-            if (elect_one()) {
-              uint32_t a_lo = a_lo0;
-              uint32_t b_lo = b_lo_base + (uint32_t)bstage * b_lo_step;
-              uint32_t bf = b_full0 + 8u * (uint32_t)bstage, be = b_empty0 + 8u * (uint32_t)bstage;
-              int bs = bstage; uint32_t bp = bphase;
-              for (int ky = 0; ky < kh; ++ky, a_lo += row_skip) {
-                for (int kx = 0; kx < kw; ++kx, a_lo += 8u) {
-                  mbar_wait(bf, bp);
-                  tc_fence_after();
-#pragma unroll
-                  for (int sub = 0; sub < S; ++sub) {
-                    const uint32_t d = tmem_d + (uint32_t)sub * bn, al = a_lo + (uint32_t)sub * 64u;
-                    for (int ks = 0; ks < nks; ++ks)
-                      tc_mma_bf16_lohi(d, al + 2u * ks, a_hi, b_lo + 2u * ks, b_hi, idesc, ks == 0 ? fresh : 1u);
-                  }
-                  tc_commit(be);
-                  fresh = 1u;
-                  b_lo += b_lo_step; bf += 8u; be += 8u;
-                  if (++bs == b_stages) { bs = 0; bp ^= 1u; b_lo = b_lo_base; bf = b_full0; be = b_empty0; }
-                }
-              }
-              tc_commit(a_empty(astage));
-            }
-            __syncwarp();
-            fresh = 1u;
-            bstage += kh * kw;
-            while (bstage >= b_stages) { bstage -= b_stages; bphase ^= 1u; }
-            if (++astage == a_stages) { astage = 0; aphase ^= 1u; }
-          }
-        }
-        if (elect_one()) tc_commit(tfull_bar(acc));
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else {
-    // ===================================== epilogue warps ================================================================
-    const int ew = warp - 3;
-    const int q = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int l = 0; l < P.nlayers; ++l) {
-      const ChainL& p = P.L[l];
-      const int nchunks = p.block_n >> 4;
-      const int items = S * nchunks;
-      const int it_begin = (ew < 4) ? 0 : ((items + 1) >> 1);
-      const int it_end = (ew < 4) ? ((items + 1) >> 1) : items;
       // bias of this layer (the previous layer's tiles of this CTA are finished: its arrival below came after them)
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int i = threadIdx.x - 96; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
+      for (int i = ct; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
       asm volatile("bar.sync 1, 256;" ::: "memory");
       if (l > 0 && p.res != nullptr) {                        // the residual may come from an earlier layer of this chain: acquire it
         if (lane == 0 && !chain_wait(P.bar + (l - 1), gridDim.x)) *P.err = 1u;
         __syncwarp();
       }
-      const float4* bias4 = reinterpret_cast<const float4*>(bias_s);
       TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = 0; ep.out = p.out; ep.res = p.res;
-      const bool fast_launch = !p.out_f32 && p.res == nullptr && p.act <= ACT_RELU && (reinterpret_cast<uintptr_t>(p.out) & 15u) == 0 &&
-                               (p.oW & 7) == 0 && (p.oH & 7) == 0 && (p.oN & 7) == 0;
-      const float slope = p.act == ACT_LEAKY ? 0.1f : (p.act == ACT_RELU ? 0.f : 1.f);
-      const int sub_begin = it_begin / nchunks, ch_begin = it_begin - sub_begin * nchunks;
-      for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-        int t = tile;
-        const int tx = t % p.tiles_x; t /= p.tiles_x;
-        const int ty = t % p.tiles_y; t /= p.tiles_y;
-        const int n = t % p.N; const int nb = t / p.N;
-        const int xs = tx * 8 * S + (lane & 7), y = ty * CHAIN_TH + 4 * q + (lane >> 3);
-        const int cbase = nb * p.block_n;
-        mbar_wait(tfull_bar(acc), acc_phase);
-        tc_fence_after();
-        const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.acc_cols);
-        const bool yin = y < p.H;
-        const long long opix0 = n * p.oN + (long long)y * p.oH + (long long)xs * p.oW, rpix0 = n * p.rN + (long long)y * p.rH + (long long)xs * p.rW;
-        int sub = sub_begin, ch = ch_begin;
-        for (int it = it_begin; it < it_end; it += 2) {
-          uint32_t v0[16], v1[16];
-          const bool two = it + 1 < it_end;
-          const int sub_a = sub, ch_a = ch;
-          if (++ch == nchunks) { ch = 0; ++sub; }
-          const int sub_b = sub, ch_b = ch;
-          if (++ch == nchunks) { ch = 0; ++sub; }
-          __syncwarp();
-          tc_ld16_nowait(taddr0 + (uint32_t)(sub_a * p.block_n + ch_a * 16), v0);
-          if (two) tc_ld16_nowait(taddr0 + (uint32_t)(sub_b * p.block_n + ch_b * 16), v1);
-          tc_ld_wait16(v0);
-          if (two) tc_ld_wait16(v1);
-          {
-            const int c = cbase + ch_a * 16;
-            const bool ok = yin && xs + 8 * sub_a < p.W;
-            if (fast_launch && c + 16 <= p.Cout)
-              tc_epilogue16_fast(v0, bias_s + c, slope, reinterpret_cast<__nv_bfloat16*>(p.out) + opix0 + (long long)(8 * sub_a) * p.oW + c, ok);
-            else if (ok && c < p.zero_pad_to)
-              tc_epilogue16_call(ep, v0, bias4, c, opix0 + (long long)(8 * sub_a) * p.oW, rpix0 + (long long)(8 * sub_a) * p.rW);
-          }
-          if (two) {
-            const int c = cbase + ch_b * 16;
-            const bool ok = yin && xs + 8 * sub_b < p.W;
-            if (fast_launch && c + 16 <= p.Cout)
-              tc_epilogue16_fast(v1, bias_s + c, slope, reinterpret_cast<__nv_bfloat16*>(p.out) + opix0 + (long long)(8 * sub_b) * p.oW + c, ok);
-            else if (ok && c < p.zero_pad_to)
-              tc_epilogue16_call(ep, v1, bias4, c, opix0 + (long long)(8 * sub_b) * p.oW, rpix0 + (long long)(8 * sub_b) * p.rW);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(acc));
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+      switch (p.block_n) {
+        case 16: chain_layer<S, 16>(p, ra, rb, ep, bias_s, wg, wq, lane, leader); break;
+        case 32: chain_layer<S, 32>(p, ra, rb, ep, bias_s, wg, wq, lane, leader); break;
+        case 64: chain_layer<S, 64>(p, ra, rb, ep, bias_s, wg, wq, lane, leader); break;
+        case 128: if (S <= 2) chain_layer<S, (S <= 2 ? 128 : 16)>(p, ra, rb, ep, bias_s, wg, wq, lane, leader); break;
+        default: if (S == 1) chain_layer<S, (S == 1 ? 256 : 16)>(p, ra, rb, ep, bias_s, wg, wq, lane, leader); break;
       }
       // this CTA's share of layer l is in global memory: publish it to the other CTAs' TMA loads
       if (l + 1 < P.nlayers) {
         asm volatile("fence.proxy.async;" ::: "memory");
         __threadfence();
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (threadIdx.x == 96) chain_arrive(P.bar + l);
+        if (ct == 0) chain_arrive(P.bar + l);
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)P.tmem_cols) : "memory");
   }
 }
 
@@ -354,8 +231,9 @@ bool conv_chain_eligible(const ConvTc& c) {
   return c.Cout_pad % 16 == 0 && c.Cout_pad <= 256;
 }
 
-// per-K16-step clocks of one M = 128 MMA with N = bn (measured: the tensor core reads its shared-memory operands at ~64 B/clk)
-static double chain_mma_clk(int bn) { return 64.0 + 0.5 * bn; }
+// per-K16-step clocks of one M = 128 MMA with N = bn: the larger of the tensor rate and the shared-memory operand reads (the
+// estimate conv_halo.cu's halo_choose uses)
+static double chain_mma_clk(int bn) { return bn > 32 + 0.5 * bn ? (double)bn : 32 + 0.5 * bn; }
 
 int conv_chain_launch(const std::vector<ConvTc>& layers, unsigned* bar, cudaStream_t s) {
   const int n = (int)layers.size();
@@ -375,7 +253,7 @@ int conv_chain_launch(const std::vector<ConvTc>& layers, unsigned* bar, cudaStre
       int k16 = 0;
       for (int i = 0; i < c.nsrc; ++i) k16 += (c.src[i].C + 15) / 16;
       double bl = -1.0; int bbn = 0;
-      for (int bn = 16; bn <= c.Cout_pad && bn <= 256; bn += 16) {
+      for (int bn = 16; bn <= c.Cout_pad && bn <= 256; bn <<= 1) {         // the wgmma shapes 16 .. 256
         if (c.Cout_pad % bn || S * bn > 256) continue;
         const long long tiles = (long long)cdiv(c.W, 8 * S) * cdiv(c.H, CHAIN_TH) * c.N * (c.Cout_pad / bn);
         const long long waves = (tiles + nsm - 1) / nsm;
@@ -396,7 +274,7 @@ int conv_chain_launch(const std::vector<ConvTc>& layers, unsigned* bar, cudaStre
   static ChainArgs A;                     // 8.5 KB of kernel parameters; filled per launch (single host thread per context)
   memset(&A, 0, sizeof(A));
   A.nlayers = n;
-  int a_stage = 0, b_stage = 0, acc_max = 0, cout_max = 0, grid = 1;
+  int a_stage = 0, b_stage = 0, cout_max = 0, grid = 1;
   double flops = 0.0;
   for (int l = 0; l < n; ++l) {
     const ConvTc& c = layers[l];
@@ -408,7 +286,6 @@ int conv_chain_launch(const std::vector<ConvTc>& layers, unsigned* bar, cudaStre
     k.n_blocks = c.Cout_pad / k.block_n;
     k.ntiles = k.tiles_x * k.tiles_y * c.N * k.n_blocks;
     k.HW = 8 * bestS + k.kw - 1; k.HH = CHAIN_TH + k.kh - 1;
-    k.acc_cols = bestS * k.block_n;
     k.nsrc = c.nsrc;
     int ktot = 0;
     for (int i = 0; i < c.nsrc; ++i) { k.srcC[i] = c.src[i].C; ktot += c.src[i].C; }
@@ -419,7 +296,6 @@ int conv_chain_launch(const std::vector<ConvTc>& layers, unsigned* bar, cudaStre
     const int as = (k.HW * k.HH * 128 + 1023) & ~1023;
     if (as > a_stage) a_stage = as;
     if (k.block_n * 128 > b_stage) b_stage = k.block_n * 128;
-    if (k.acc_cols > acc_max) acc_max = k.acc_cols;
     if (c.Cout_pad > cout_max) cout_max = c.Cout_pad;
     if (k.ntiles > grid) grid = k.ntiles;
     flops += c.flops;
@@ -442,7 +318,7 @@ int conv_chain_launch(const std::vector<ConvTc>& layers, unsigned* bar, cudaStre
   }
   if (grid > nsm) grid = nsm;
   // ring geometry common to the chain
-  const size_t fixed = 1024 + 8 * 64 + 64 + (size_t)cout_max * 4;
+  const size_t fixed = 1024 + 8 * 64 + (size_t)cout_max * 4;
   const size_t budget = 220 * 1024;
   int a_stages = 2, b_stages = 2;
   DFVO_REQUIRE(fixed + 2 * (size_t)a_stage + 2 * (size_t)b_stage <= budget, DFVO_EINVAL, "conv_chain: tiles do not fit in shared memory");
@@ -450,8 +326,7 @@ int conv_chain_launch(const std::vector<ConvTc>& layers, unsigned* bar, cudaStre
   while (a_stages < 3 && fixed + (size_t)(a_stages + 1) * a_stage + (size_t)b_stages * b_stage <= budget) ++a_stages;
   while (b_stages < 12 && fixed + (size_t)a_stages * a_stage + (size_t)(b_stages + 1) * b_stage <= budget) ++b_stages;
   A.a_stages = a_stages; A.b_stages = b_stages; A.a_stage_bytes = a_stage; A.b_stage_bytes = b_stage;
-  int cols = 32; while (cols < 2 * acc_max) cols <<= 1;
-  A.tmem_cols = cols; A.bias_cap = cout_max;
+  A.bias_cap = cout_max;
   const size_t smem = fixed + (size_t)a_stages * a_stage + (size_t)b_stages * b_stage;
   // arrival counters: CHAIN_BAR_WORDS words owned by the caller (one block per chain site of a network, so launches that may be in
   // flight together -- other engines, other graphs -- never share counters); word [CHAIN_MAXL] collects the watchdog flag

@@ -1,5 +1,5 @@
 // CUDA-core implicit-GEMM convolution (fp32 accumulate), NHWC, any kernel size / stride, zero or
-// reflection padding, fused bias + activation + residual.  Used for the layers the tcgen05 kernel
+// reflection padding, fused bias + activation + residual.  Used for the layers the wgmma kernel
 // does not cover (3-channel 7x7 stems, stride-2 convs, 1-channel heads) and for the all-fp32
 // "exact" mode the parity tests use.  Restates torch.nn.Conv2d as used at lite_flow_net.py:39-75
 // and resnet_encoder.py / layers.py:121-136 (ReflectionPad2d(1) + 3x3).

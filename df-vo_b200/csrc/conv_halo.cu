@@ -1,19 +1,19 @@
-// Halo-resident tcgen05 implicit-GEMM convolution for sm_100a (stride 1, rectangular kh x kw tap set, up to 3
-// virtually concatenated NHWC bf16 sources, fused bias + activation + residual epilogue).
+// Halo-resident wgmma implicit-GEMM convolution for sm_90a (stride 1, rectangular kh x kw tap set, up to 3 virtually
+// concatenated NHWC bf16 / fp32 sources, fused bias + activation + residual epilogue).
 //
-// Why a second kernel: conv_tc.cu loads one shifted A box per tap, so a 3x3 layer pulls every input pixel nine
-// times and the full weight set once per 128 output pixels through L2 -> SM.  The chip-wide L2 output cap
-// (~6.3 KB/clk, B300_MICROARCH.md "LTS throughput cap"; ~43 B/clk per SM) then bounds the layer at ~1/3 of the
-// tensor peak (measured: 370 MB of xbar->SM traffic for 22 MB of input on the 194->128 layer).  Here
+// Why a second kernel: conv_tc.cu loads one shifted A box per tap, so a 3x3 layer pulls every input pixel nine times and the
+// full weight set once per 128 output pixels through L2 -> SM, and L2 bandwidth bounds such a layer well below the tensor rate.
+// Here
 //   * the A operand of a tile is ONE TMA box per 64-channel chunk: the (8S + kw - 1) x (16 + kh - 1) pixel halo
 //     of the tile, 128 B per pixel, SWIZZLE_128B.  Every tap of the kh x kw window is the same shared-memory
-//     data addressed through a UMMA descriptor whose start is shifted by (ky * halo_w + kx) pixels and whose
+//     data addressed through a wgmma descriptor whose start is shifted by (ky * halo_w + kx) pixels and whose
 //     stride-byte-offset is one halo row: the 8-row groups of the K-major operand are the tile's pixel rows.
 //     A 3x3 layer reads each input pixel 1.27x (S = 2) instead of 9x;
 //   * one CTA owns S sub-tiles of 8 x 16 pixels (M = 128 each) that share every B (weight) stage, so the
-//     weights cross L2 -> SM once per 128*S pixels; accumulators: S x block_n TMEM columns, double buffered;
+//     weights cross L2 -> SM once per 128*S pixels;
 //   * A and B have their own mbarrier rings and producer warps (a B slot is freed per tap, an A slot per chunk).
-// Warp roles: 0 = A producer (TMA), 1 = B producer (TMA), 2 = MMA issuer + TMEM owner, 3..10 = epilogue.
+// Warp roles: 0 = A producer (TMA), 1 = B producer (TMA), 2-3 idle; warpgroups 1 and 2 = consumers (wgmma for pixel rows 0-7 / 8-15
+// of every sub-tile, accumulators in registers, then the epilogue).  tc_ptx.cuh::halo_tile_mma is the MMA loop.
 // Restates torch.nn.Conv2d(stride=1) + LeakyReLU/ELU/ReLU as used at lite_flow_net.py:98-240 and
 // depth_decoder.py / torchvision BasicBlock (BN folded by the weight packer), like conv_tc.cu.
 #include "tc_ptx.cuh"
@@ -28,87 +28,57 @@ namespace dfvo {
 
 struct ConvHaloK {
   int N, H, W, tiles_x, tiles_y, n_blocks, ntiles;
-  int S;                         // sub-tiles (8 px wide, 16 px high) per tile
   int nsrc, srcC[3];
   int kh, kw, dy0, dx0;          // input pixel of tap (ky,kx) for output (y,x): (y + dy0 + ky, x + dx0 + kx)
   int HW, HH;                    // halo box, pixels
-  int block_n, a_stages, b_stages, a_stage_bytes, acc_cols, tmem_cols;
+  int a_stages, b_stages, a_stage_bytes;
   int Cout, Cout_pad, act, out_f32, zero_pad_to;
   int chunk;                     // channels per 128-byte operand row: 64 (bf16) or 32 (fp32 read as tf32)
   int esize, round_tf32;
-  int tma_out;                   // bf16 output through shared-memory staging + cp.async.bulk.tensor stores (full-line writes)
-  int cw;                        // channels per store box: min(block_n, 64)
-  uint32_t stage_out_off;        // byte offset of the two staging buffers from the 1024-B aligned base
-  long long* dbg;                // optional per-phase clock stamps of CTA 0 (DFVO_HALO_DBG)
   const float* bias;
   void* out; long long oN, oH, oW;
   const void* res; long long rN, rH, rW;
 };
 
-#define HALO_THREADS 352
+#define HALO_THREADS 384
 #define HALO_TH 16
 
-template <int S, int TF32>
+template <int S, int BN, int TF32>
 __global__ void __launch_bounds__(HALO_THREADS, 1)
 k_conv_halo(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
             const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmO, const __grid_constant__ ConvHaloK p) {
+            const __grid_constant__ ConvHaloK p) {
   using namespace tc;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B pattern repeats every 1024 B
   uint8_t* base_ptr = smem_raw + (base - raw);
-  const uint32_t b_stage_bytes = (uint32_t)p.block_n * 128u;
+  const uint32_t b_stage_bytes = (uint32_t)BN * 128u;
   const uint32_t a_base = base;
   const uint32_t b_base = base + (uint32_t)p.a_stages * (uint32_t)p.a_stage_bytes;
-  // [A ring][B ring][2 store-staging boxes (tma_out)][barriers, TMEM slot, bias]
-  const uint32_t bar_base = b_base + (uint32_t)p.b_stages * b_stage_bytes + (p.tma_out ? 2u * 128u * (uint32_t)p.cw * 2u : 0u);
-  // barriers: a_full[A], a_empty[A], b_full[B], b_empty[B], tmem_full[2], tmem_empty[2]
-  auto a_full = [&](int s) { return bar_base + 8u * (uint32_t)s; };
-  auto a_empty = [&](int s) { return bar_base + 8u * (uint32_t)(p.a_stages + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (uint32_t)(2 * p.a_stages + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (uint32_t)(2 * p.a_stages + p.b_stages + s); };
-  const int nbar0 = 2 * p.a_stages + 2 * p.b_stages;
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (uint32_t)(nbar0 + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (uint32_t)(nbar0 + 2 + a); };
-  uint8_t* after_bars = base_ptr + (bar_base - base) + 8u * (uint32_t)(nbar0 + 4);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(after_bars);
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 4);
+  // [A ring][B ring][barriers: a_full[A], a_empty[A], b_full[B], b_empty[B]][bias]
+  const uint32_t bar_base = b_base + (uint32_t)p.b_stages * b_stage_bytes;
+  TcRing ra{a_base, (uint32_t)p.a_stage_bytes, bar_base, bar_base + 8u * (uint32_t)p.a_stages, p.a_stages, 0, 0u};
+  TcRing rb{b_base, b_stage_bytes, bar_base + 16u * (uint32_t)p.a_stages, bar_base + 16u * (uint32_t)p.a_stages + 8u * (uint32_t)p.b_stages,
+            p.b_stages, 0, 0u};
+  float* bias_s = reinterpret_cast<float*>(base_ptr + (bar_base - base) + 16u * (uint32_t)(p.a_stages + p.b_stages));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // phase stamps (debug): 0 entry, 1 after set-up sync, 2 after the PDL wait, 3 first A box landed, 4 first accumulator complete,
-  // 5 first tile stored, 6 last tile stored (CTA 0 only; %globaltimer ns)
-  auto stamp = [&](int i) {
-    if (p.dbg && blockIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); p.dbg[i] = (long long)t; }
-  };
-  if (threadIdx.x == 0) stamp(0);
 
   pdl_trigger();
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA0); prefetch_tmap(&tmB);
-    if (p.tma_out) prefetch_tmap(&tmO);
-    for (int s = 0; s < p.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 1); }
-    for (int s = 0; s < p.b_stages; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 8); }
+    for (int s = 0; s < p.a_stages; ++s) { mbar_init(ra.full0 + 8u * s, 1); mbar_init(ra.empty0 + 8u * s, 2); }
+    for (int s = 0; s < p.b_stages; ++s) { mbar_init(rb.full0 + 8u * s, 1); mbar_init(rb.empty0 + 8u * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int ntaps = p.kh * p.kw;
-  if (threadIdx.x == 0) stamp(1);
   pdl_wait();                                  // from here on: activations of the previous kernel / our output buffers
-  if (threadIdx.x == 0) stamp(2);
 
   if (warp == 0) {
     // ===================================== A producer: one halo box per (tile, source, 64-channel chunk)
-    int stage = 0; uint32_t phase = 0;
     const uint32_t a_bytes = (uint32_t)p.HW * (uint32_t)p.HH * 128u;
     for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
       int t = tile;
@@ -119,256 +89,53 @@ k_conv_halo(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CU
       for (int s = 0; s < p.nsrc; ++s) {
         const CUtensorMap* tm = s == 0 ? &tmA0 : (s == 1 ? &tmA1 : &tmA2);
         for (int c0 = 0; c0 < p.srcC[s]; c0 += p.chunk) {
-          mbar_wait(a_empty(stage), phase ^ 1u);
+          mbar_wait(ra.empty(), ra.ph ^ 1u);
           if (elect_one()) {
-            mbar_expect_tx(a_full(stage), a_bytes);
-            tma_load_4d(a_base + (uint32_t)stage * (uint32_t)p.a_stage_bytes, tm, a_full(stage), c0, x0, y0, n);
+            mbar_expect_tx(ra.full(), a_bytes);
+            tma_load_4d(ra.slot(), tm, ra.full(), c0, x0, y0, n);
           }
           __syncwarp();
-          if (++stage == p.a_stages) { stage = 0; phase ^= 1u; }
+          ra.next();
         }
       }
     }
   } else if (warp == 1) {
     // ===================================== B producer: one weight box per (tile, chunk, tap)
-    int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
       const int nb = tile / (p.tiles_x * p.tiles_y * p.N);
       int kofs = 0;
       for (int s = 0; s < p.nsrc; ++s) {
         for (int c0 = 0; c0 < p.srcC[s]; c0 += p.chunk) {
           for (int tap = 0; tap < ntaps; ++tap) {
-            mbar_wait(b_empty(stage), phase ^ 1u);
+            mbar_wait(rb.empty(), rb.ph ^ 1u);
             if (elect_one()) {
-              mbar_expect_tx(b_full(stage), b_stage_bytes);
-              tma_load_3d(b_base + (uint32_t)stage * b_stage_bytes, &tmB, b_full(stage), kofs + c0, nb * p.block_n, tap);
+              mbar_expect_tx(rb.full(), b_stage_bytes);
+              tma_load_3d(rb.slot(), &tmB, rb.full(), kofs + c0, nb * BN, tap);
             }
             __syncwarp();
-            if (++stage == p.b_stages) { stage = 0; phase ^= 1u; }
+            rb.next();
           }
         }
         kofs += p.srcC[s];
       }
     }
-  } else if (warp == 2) {
-    // ===================================== MMA issuer =========================================
-    // The warp walks tiles and chunks together; inside a chunk ONE elected lane waits for each B slot and issues that
-    // tap's S*4 MMAs + the commit.  The per-tap instruction stream is kept to a few uniform-datapath operations (every
-    // loop invariant lives in a register, descriptors advance by adds): a single thread issues dependent instructions
-    // ~4-8 clk apart, and an N = 64 MMA is only 32 tensor clocks long, so a fat loop body starves the tensor pipe
-    // (measured: 50 % tensor-pipe activity with ~130 instructions per tap, MMA warp never waiting for data).
-    const uint32_t idesc = tc_idesc(TF32, p.block_n);
-    // descriptor words: lo = start>>4 [0,14) | LBO (unused for swizzled K-major, 1) [16,30);
-    //                   hi = SBO>>4 [0,14) | version 1 [14,16) | SWIZZLE_128B (2) [29,32).  A: SBO = one halo row; B: 1024 B
-    const uint32_t a_hi = (((uint32_t)p.HW * 128u) >> 4) | (1u << 14) | (2u << 29);
-    const uint32_t b_hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-    // base_offset stays 0: the swizzle pattern (written by TMA) starts at the 1024-B aligned stage base and the tensor
-    // core applies the XOR to absolute shared-memory addresses, so a start shifted by whole 128-B pixel rows and an
-    // SBO that is not a multiple of 1024 B address exactly the bytes TMA wrote (validated on B200 against an fp64
-    // convolution for S = 1, 2, 4; base_offset = (start >> 7) & 7 gives wrong results)
-    const int kh = p.kh, kw = p.kw, a_stages = p.a_stages, b_stages = p.b_stages;
-    const uint32_t row_skip = (uint32_t)(p.HW - p.kw) * 8u;        // from the end of one tap row to the next, 16-B units
-    const uint32_t bn = (uint32_t)p.block_n;
-    const uint32_t b_lo_base = ((b_base >> 4) & 0x3FFFu) | (1u << 16), b_lo_step = b_stage_bytes >> 4;
-    const uint32_t b_full0 = b_full(0), b_empty0 = b_empty(0);
-    int astage = 0; uint32_t aphase = 0;
-    int bstage = 0; uint32_t bphase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * p.acc_cols);
-      uint32_t fresh = 0;                         // 0 for the first (chunk, tap) of the tile: its ks = 0 MMAs overwrite
-      for (int s = 0; s < p.nsrc; ++s) {
-        for (int c0 = 0; c0 < p.srcC[s]; c0 += p.chunk) {
-          mbar_wait(a_full(astage), aphase);
-          tc_fence_after();
-          if (p.dbg && tile == (int)blockIdx.x && s == 0 && c0 == 0 && lane == 0) stamp(3);
-          const uint32_t a_lo0 = (((a_base + (uint32_t)astage * (uint32_t)p.a_stage_bytes) >> 4) & 0x3FFFu) | (1u << 16);
-          const int rem = p.srcC[s] - c0;
-          const int nks = ((rem >= p.chunk ? p.chunk : rem) * p.esize) >> 5;       // 32-byte K steps (16 bf16 / 8 tf32) with real channels
-          if (elect_one()) {
-            uint32_t a_lo = a_lo0;                             // + (ky * HW + kx) pixels * 128 B, in 16-B units
-            uint32_t b_lo = b_lo_base + (uint32_t)bstage * b_lo_step;
-            uint32_t bf = b_full0 + 8u * (uint32_t)bstage, be = b_empty0 + 8u * (uint32_t)bstage;
-            int bs = bstage; uint32_t bp = bphase;
-            for (int ky = 0; ky < kh; ++ky, a_lo += row_skip) {
-              for (int kx = 0; kx < kw; ++kx, a_lo += 8u) {
-                mbar_wait(bf, bp);
-                tc_fence_after();
-                if (nks == 4) {
-#pragma unroll
-                  for (int sub = 0; sub < S; ++sub) {
-                    const uint32_t d = tmem_d + (uint32_t)sub * bn, al = a_lo + (uint32_t)sub * 64u;            // +8 pixels
-                    tc_mma_lohi<TF32>(d, al, a_hi, b_lo, b_hi, idesc, fresh);
-                    tc_mma_lohi<TF32>(d, al + 2u, a_hi, b_lo + 2u, b_hi, idesc, 1u);       // +32 B inside the swizzle atom
-                    tc_mma_lohi<TF32>(d, al + 4u, a_hi, b_lo + 4u, b_hi, idesc, 1u);
-                    tc_mma_lohi<TF32>(d, al + 6u, a_hi, b_lo + 6u, b_hi, idesc, 1u);
-                  }
-                } else {
-#pragma unroll
-                  for (int sub = 0; sub < S; ++sub) {
-                    const uint32_t d = tmem_d + (uint32_t)sub * bn, al = a_lo + (uint32_t)sub * 64u;
-                    for (int ks = 0; ks < nks; ++ks)
-                      tc_mma_lohi<TF32>(d, al + 2u * ks, a_hi, b_lo + 2u * ks, b_hi, idesc, ks == 0 ? fresh : 1u);
-                  }
-                }
-                tc_commit(be);
-                fresh = 1u;
-                b_lo += b_lo_step; bf += 8u; be += 8u;
-                if (++bs == b_stages) { bs = 0; bp ^= 1u; b_lo = b_lo_base; bf = b_full0; be = b_empty0; }
-              }
-            }
-            tc_commit(a_empty(astage));
-          }
-          __syncwarp();
-          fresh = 1u;
-          // every lane tracks the B ring position (kh*kw slots consumed by the elected lane)
-          bstage += kh * kw;
-          while (bstage >= b_stages) { bstage -= b_stages; bphase ^= 1u; }
-          if (++astage == a_stages) { astage = 0; aphase ^= 1u; }
-        }
-      }
-      if (elect_one()) tc_commit(tfull_bar(acc));
-      __syncwarp();
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
-  } else {
-    // ===================================== epilogue warps ====================================
-    // 8 warps: TMEM lane quadrant = warp % 4 (hardware rule); the two warps of a quadrant split the
-    // (sub-tile, 16-column chunk) items.  Lane -> pixel (x = lane % 8, y = 4 * quadrant + lane / 8) of a sub-tile.
-    const int ew = warp - 3;
-    const int q = warp & 3;
-    const int nchunks = p.block_n >> 4;
-    const int items = S * nchunks;
-    const int it_begin = (ew < 4) ? 0 : ((items + 1) >> 1);
-    const int it_end = (ew < 4) ? ((items + 1) >> 1) : items;
-    // bias staging belongs to the epilogue warps alone (they idle until the first accumulator is ready anyway), so the
-    // producers and the MMA warp start on the barrier-init sync instead of waiting for a global load: ~1 us off the
-    // critical path of each of the ~115 launches per frame.
-    for (int i = threadIdx.x - 96; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
+  } else if (warp >= 4) {
+    // ============================ two consumer warpgroups: MMA + epilogue ============================
+    const int ct = threadIdx.x - 128, wg = ct >> 7;
+    // bias staging belongs to the consumers (the producers start on the barrier-init sync instead of waiting for a global load)
+    for (int i = ct; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
     asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float4* bias4 = reinterpret_cast<const float4*>(bias_s);
     TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = p.round_tf32; ep.out = p.out; ep.res = p.res;
-    int acc = 0; uint32_t acc_phase = 0;
-    uint32_t store_seq = 0;
-    // lean path: bf16 output, no residual, LeakyReLU / ReLU / identity, 16-byte aligned pixels (uniform per launch)
-    const bool fast_launch = !p.out_f32 && p.res == nullptr && p.act <= ACT_RELU && (reinterpret_cast<uintptr_t>(p.out) & 15u) == 0 &&
-                             (p.oW & 7) == 0 && (p.oH & 7) == 0 && (p.oN & 7) == 0;
-    const float slope = p.act == ACT_LEAKY ? 0.1f : (p.act == ACT_RELU ? 0.f : 1.f);      // max(f, slope * f); identity: max(f, f)
-    const int sub_begin = it_begin / nchunks, ch_begin = it_begin - sub_begin * nchunks;
+    float acc[S][BN / 2];
     for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+      halo_tile_mma<S, BN, TF32>(acc, ra, rb, p.nsrc, p.srcC, p.chunk, p.esize, p.kh, p.kw, p.HW, wg, (ct & 127) == 0);
       int t = tile;
       const int tx = t % p.tiles_x; t /= p.tiles_x;
       const int ty = t % p.tiles_y; t /= p.tiles_y;
       const int n = t % p.N; const int nb = t / p.N;
-      const int xs = tx * 8 * S + (lane & 7), y = ty * HALO_TH + 4 * q + (lane >> 3);
-      const int cbase = nb * p.block_n;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.acc_cols);
-
-      if (p.dbg && tile == (int)blockIdx.x && threadIdx.x == 96) stamp(4);
-      if (p.tma_out) {
-        // ---- staged stores: per (sub-tile, cw-channel group) the 8 warps write their 16-column chunks of the 128 pixels into a
-        // swizzled [16 rows][8 px][cw ch] box in shared memory; one thread hands it to TMA, which writes whole lines and clips the
-        // box at the image / channel borders.  Two boxes in flight (double-buffered staging).
-        const int cw = p.cw, groups_per_sub = p.block_n / cw, ngroups = S * groups_per_sub;
-        const int chunks_per_group = cw >> 4;                              // 16-column chunks of a group: 4, 2 or 1
-        const uint32_t row_bytes = (uint32_t)cw * 2u, box_bytes = 128u * row_bytes;
-        const int sw_shift = cw == 64 ? 0 : (cw == 32 ? 1 : 2), sw_mask = cw == 64 ? 7 : (cw == 32 ? 3 : 1);
-        const int row = (4 * q + (lane >> 3)) * 8 + (lane & 7);             // this lane's pixel inside the 8 x 16 box
-        for (int g = 0; g < ngroups; ++g) {
-          const int sub = g / groups_per_sub, cg = g - sub * groups_per_sub;
-          const uint32_t buf = base + p.stage_out_off + (uint32_t)(store_seq & 1) * box_bytes;
-          if (threadIdx.x == 96) bulk_wait_read<1>();                       // the box that used this buffer two stores ago was read
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          // the two warps of a quadrant split the group's chunks
-          const int ch0 = (ew < 4) ? 0 : ((chunks_per_group + 1) >> 1), ch1 = (ew < 4) ? ((chunks_per_group + 1) >> 1) : chunks_per_group;
-          for (int ch = ch0; ch < ch1; ++ch) {
-            uint32_t v[16], w[8];
-            __syncwarp();
-            tc_ld16(taddr0 + (uint32_t)(sub * p.block_n + cg * cw + ch * 16), v);
-            {
-              const int c = cbase + cg * cw + ch * 16;
-              tc_epilogue16_fast_pack(v, bias_s + c, slope, w);                 // bias is zero-padded to Cout_pad
-              if (c + 16 > p.Cout) {                                             // channel tail: zeros beyond Cout
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const int c2 = c + 2 * j;
-                  w[j] = c2 + 1 < p.Cout ? w[j] : (c2 < p.Cout ? (w[j] & 0xffffu) : 0u);
-                }
-              }
-            }
-            const uint32_t a0 = buf + (uint32_t)row * row_bytes;
-            const int k0 = 2 * ch, sx = (row >> sw_shift) & sw_mask;       // 16-byte units inside the row, XOR-swizzled like the tensor map
-            st_shared_v4(a0 + (uint32_t)(((k0) ^ sx) << 4), w[0], w[1], w[2], w[3]);
-            st_shared_v4(a0 + (uint32_t)(((k0 + 1) ^ sx) << 4), w[4], w[5], w[6], w[7]);
-          }
-          if (g == ngroups - 1) {                                           // accumulator fully read: give it back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));
-          }
-          fence_async_smem();
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (threadIdx.x == 96) {
-            tma_store_4d(&tmO, buf, cbase + cg * cw, tx * 8 * S + 8 * sub, ty * HALO_TH, n);
-            bulk_commit();
-          }
-          ++store_seq;
-        }
-        if (p.dbg && threadIdx.x == 96) stamp(tile == (int)blockIdx.x ? 5 : 6);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-        continue;
-      }
-      // two items (sub-tile, 16-column chunk) in flight; (sub, ch) advance without divisions
-      const bool yin = y < p.H;
-      const long long opix0 = n * p.oN + (long long)y * p.oH + (long long)xs * p.oW, rpix0 = n * p.rN + (long long)y * p.rH + (long long)xs * p.rW;
-      int sub = sub_begin, ch = ch_begin;
-      for (int it = it_begin; it < it_end; it += 2) {
-        uint32_t v0[16], v1[16];
-        const bool two = it + 1 < it_end;
-        const int sub_a = sub, ch_a = ch;
-        if (++ch == nchunks) { ch = 0; ++sub; }
-        const int sub_b = sub, ch_b = ch;
-        if (++ch == nchunks) { ch = 0; ++sub; }
-        __syncwarp();                              // tcgen05.ld is .sync.aligned: reconverge first
-        tc_ld16_nowait(taddr0 + (uint32_t)(sub_a * p.block_n + ch_a * 16), v0);
-        if (two) tc_ld16_nowait(taddr0 + (uint32_t)(sub_b * p.block_n + ch_b * 16), v1);
-        tc_ld_wait16(v0);
-        if (two) tc_ld_wait16(v1);
-        {
-          const int c = cbase + ch_a * 16;
-          const bool ok = yin && xs + 8 * sub_a < p.W;
-          if (fast_launch && c + 16 <= p.Cout)
-            tc_epilogue16_fast(v0, bias_s + c, slope, reinterpret_cast<__nv_bfloat16*>(p.out) + opix0 + (long long)(8 * sub_a) * p.oW + c, ok);
-          else if (ok && c < p.zero_pad_to)
-            tc_epilogue16_call(ep, v0, bias4, c, opix0 + (long long)(8 * sub_a) * p.oW, rpix0 + (long long)(8 * sub_a) * p.rW);
-        }
-        if (two) {
-          const int c = cbase + ch_b * 16;
-          const bool ok = yin && xs + 8 * sub_b < p.W;
-          if (fast_launch && c + 16 <= p.Cout)
-            tc_epilogue16_fast(v1, bias_s + c, slope, reinterpret_cast<__nv_bfloat16*>(p.out) + opix0 + (long long)(8 * sub_b) * p.oW + c, ok);
-          else if (ok && c < p.zero_pad_to)
-            tc_epilogue16_call(ep, v1, bias4, c, opix0 + (long long)(8 * sub_b) * p.oW, rpix0 + (long long)(8 * sub_b) * p.rW);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (p.dbg && threadIdx.x == 96) stamp(tile == (int)blockIdx.x ? 5 : 6);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+      halo_tile_store<S, BN>(acc, ep, bias_s, nb * BN, n, tx * 8 * S, ty * HALO_TH, p.W, p.H, p.oN, p.oH, p.oW, p.rN, p.rH, p.rW, wg,
+                             (ct >> 5) & 3, lane);
     }
-    if (p.tma_out && threadIdx.x == 96) bulk_wait_all();                  // global writes of every box performed before the grid ends
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
   }
 }
 
@@ -399,18 +166,17 @@ static bool rect_taps(const ConvTc& c, int* kh, int* kw, int* dy0, int* dx0) {
 
 struct HaloCfg { int S, block_n, a_stages, b_stages, a_stage_bytes; size_t smem; double cost; };
 
-// shared memory: A ring + B ring + barriers + TMEM slot + bias (+ 1 KB alignment slack)
-static bool halo_fit(int S, int bn, int kh, int kw, int Cout_pad, bool tma_out, HaloCfg* out) {
+// shared memory: A ring + B ring + barriers + bias (+ 1 KB alignment slack)
+static bool halo_fit(int S, int bn, int kh, int kw, int Cout_pad, HaloCfg* out) {
   const int HW = 8 * S + kw - 1, HH = HALO_TH + kh - 1;
   if (HW > 256 || HH > 256) return false;
   const int a_stage = (HW * HH * 128 + 1023) & ~1023;
   const int b_stage = bn * 128;
-  const size_t staging = tma_out ? 2 * 128 * (size_t)(bn < 64 ? bn : 64) * 2 : 0;      // two store boxes of 128 px x min(bn, 64) bf16
-  const size_t fixed = 1024 + 8 * 64 + 64 + (size_t)Cout_pad * 4 + staging;      // alignment slack, <= 34 barriers, TMEM slot, bias
+  const size_t fixed = 1024 + 8 * 64 + (size_t)Cout_pad * 4;      // alignment slack, <= 30 barriers, bias
   const size_t budget = 220 * 1024;
   int a_stages = 2, b_stages = 2;
   if (fixed + (size_t)a_stages * a_stage + (size_t)b_stages * b_stage > budget) return false;
-  // a B slot lives for one tap (S*4 MMAs), an A slot for a whole chunk (kh*kw taps): two A slots already cover the
+  // a B slot lives for one tap (S MMAs per K step), an A slot for a whole chunk (kh*kw taps): two A slots already cover the
   // TMA latency, so the B ring grows first (up to 8 slots in flight), then a third A slot, then B up to 12
   while (b_stages < 8 && fixed + (size_t)a_stages * a_stage + (size_t)(b_stages + 1) * b_stage <= budget) ++b_stages;
   while (a_stages < 3 && fixed + (size_t)(a_stages + 1) * a_stage + (size_t)b_stages * b_stage <= budget) ++a_stages;
@@ -420,18 +186,11 @@ static bool halo_fit(int S, int bn, int kh, int kw, int Cout_pad, bool tma_out, 
   return true;
 }
 
-// Pick (S, block_n): minimise  waves x max(MMA time, L2->SM time)  per tile + a fixed per-tile overhead.
-// MMA time per K=16 step = max(block_n/2, 32 + block_n/4) clk (tensor floor vs shared-memory operand reads),
-// L2->SM ~ 43 B/clk per SM when every SM streams (chip cap 6.3 KB/clk), up to ~3x that for a lone CTA.
-static bool halo_tma_out(const ConvTc& c) {
-  static int on = -1;
-  // opt-in: measured on B200 (profiles/r02_trace_tma_store.txt) the staged TMA-store epilogue is SLOWER than direct 2 x 16-byte stores on
-  // every full-channel layer (1x1 32->64 @176x608: 26.8 vs 22.7 us; the epilogue is instruction-issue bound, not store bound, and the
-  // staging adds two named barriers + a proxy fence per box); it only wins on the 9 / 25-channel distance maps (11 vs 13 us)
-  if (on < 0) on = env_int("DFVO_TMA_STORE", 0);
-  return on && !c.out_f32 && c.residual == nullptr && c.act <= ACT_RELU && ((uintptr_t)c.out & 15) == 0 && (c.oW * 2) % 16 == 0 && (c.oH * 2) % 16 == 0 && (c.oN * 2) % 16 == 0;
-}
-
+// Pick (S, block_n): minimise  waves x max(MMA time, L2->SM time)  per tile + a fixed per-tile overhead.  An estimate from the
+// H100 SXM data sheet, not a measurement: per K=16 step of the 128-pixel sub-tile, MMA time = max(block_n, 32 + block_n / 2) clk
+// (tensor rate of ~2048 bf16 MACs / clk / SM vs shared-memory operand reads at 128 B / clk); L2 -> SM ~25 B/clk per SM when every
+// SM streams (~3.3 KB / clk for the chip), up to ~5x that for a lone CTA.  block_n is one of the wgmma shapes 16 .. 256 and
+// S * block_n <= 256 keeps the accumulators of a consumer thread at <= 128 registers.
 static bool halo_choose(const ConvTc& c, int kh, int kw, HaloCfg* best) {
   int ktot16 = 0, kbytes = 0;                       // 32-byte K steps and bytes per pixel over all sources
   const int es = c.esize == 4 ? 4 : 2;
@@ -441,21 +200,20 @@ static bool halo_choose(const ConvTc& c, int kh, int kw, HaloCfg* best) {
   bool found = false;
   for (int S = 1; S <= 4; S <<= 1) {
     if (fS && S != fS) continue;
-    for (int bn = 16; bn <= 256 && bn <= c.Cout_pad; bn += 16) {
+    for (int bn = 16; bn <= 256 && bn <= c.Cout_pad; bn <<= 1) {
       if (c.Cout_pad % bn || S * bn > 256) continue;
       if (fN && bn != fN) continue;
       HaloCfg h;
-      if (!halo_fit(S, bn, kh, kw, c.Cout_pad, halo_tma_out(c), &h)) continue;
+      if (!halo_fit(S, bn, kh, kw, c.Cout_pad, &h)) continue;
       const long long tiles = (long long)cdiv(c.W, 8 * S) * cdiv(c.H, HALO_TH) * c.N * (c.Cout_pad / bn);
       const long long waves = (tiles + nsm - 1) / nsm;
       const int active = (int)(tiles < nsm ? tiles : nsm);
-      const double mma = (double)ktot16 * kh * kw * S * ((bn / 2.0 > 32 + bn / 4.0) ? bn / 2.0 : 32 + bn / 4.0);
+      const double mma = (double)ktot16 * kh * kw * S * ((bn > 32 + bn / 2.0) ? bn : 32 + bn / 2.0);
       const double bytes = (double)(8 * S + kw - 1) * (HALO_TH + kh - 1) * kbytes + (double)kh * kw * bn * kbytes;
-      double bw = 6300.0 / active; if (bw > 128.0) bw = 128.0;
+      double bw = 3300.0 / active; if (bw > 128.0) bw = 128.0;
       const double l2 = bytes / bw;
-      const double epi = (double)S * bn * 10.0;                 // ~epilogue clk per tile (hidden unless it dominates)
-      double tile = mma > l2 ? mma : l2;
-      if (epi > tile) tile = epi;
+      const double epi = (double)S * bn * 10.0;                 // ~epilogue clk per tile (not overlapped with the MMAs)
+      const double tile = (mma > l2 ? mma : l2) + epi;
       h.cost = (double)waves * (tile + 1500.0) + 4000.0;        // per-tile pipeline bubble, per-launch prologue
       if (!found || h.cost < best->cost) { *best = h; found = true; }
     }
@@ -472,6 +230,30 @@ bool conv_halo_supported(const ConvTc& c) {
   return halo_choose(c, kh, kw, &h);
 }
 
+template <int S, int BN, int TF32>
+static int launch_halo(const CUtensorMap* tmA, const CUtensorMap& tmB, const ConvHaloK& k, int grid, size_t smem, cudaStream_t s) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<S, BN, TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  cudaLaunchConfig_t cfg; cudaLaunchAttribute attr;
+  tc_launch_config(&cfg, &attr, grid, HALO_THREADS, smem, s);
+  DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<S, BN, TF32>, tmA[0], tmA[1], tmA[2], tmB, k));
+  return DFVO_OK;
+}
+
+template <int TF32>
+static int launch_halo_t(int S, int bn, const CUtensorMap* tmA, const CUtensorMap& tmB, const ConvHaloK& k, int grid, size_t smem,
+                         cudaStream_t s) {
+#define DFVO_HALO_CASE(SS, NN) if (S == SS && bn == NN) return launch_halo<SS, NN, TF32>(tmA, tmB, k, grid, smem, s);
+  DFVO_HALO_CASE(1, 16) DFVO_HALO_CASE(1, 32) DFVO_HALO_CASE(1, 64) DFVO_HALO_CASE(1, 128) DFVO_HALO_CASE(1, 256)
+  DFVO_HALO_CASE(2, 16) DFVO_HALO_CASE(2, 32) DFVO_HALO_CASE(2, 64) DFVO_HALO_CASE(2, 128)
+  DFVO_HALO_CASE(4, 16) DFVO_HALO_CASE(4, 32) DFVO_HALO_CASE(4, 64)
+#undef DFVO_HALO_CASE
+  DFVO_REQUIRE(false, DFVO_EINVAL, "conv_halo: no kernel for S %d block_n %d", S, bn);
+}
+
 int conv_halo(const ConvTc& c, cudaStream_t s) {
   DFVO_REQUIRE(c.nsrc >= 1 && c.nsrc <= 3 && c.ntaps >= 1 && c.ntaps <= 49, DFVO_EINVAL, "conv_halo: nsrc/ntaps");
   DFVO_REQUIRE(c.Cout_pad % 16 == 0 && c.Cout_pad >= 16, DFVO_EINVAL, "conv_halo: Cout_pad %d must be a multiple of 16", c.Cout_pad);
@@ -480,15 +262,13 @@ int conv_halo(const ConvTc& c, cudaStream_t s) {
   DFVO_REQUIRE(rect_taps(c, &k.kh, &k.kw, &k.dy0, &k.dx0), DFVO_EINVAL, "conv_halo: taps are not a rectangle");
   HaloCfg h;
   DFVO_REQUIRE(halo_choose(c, k.kh, k.kw, &h), DFVO_EINVAL, "conv_halo: no tile configuration fits");
-  k.N = c.N; k.H = c.H; k.W = c.W; k.S = h.S; k.block_n = h.block_n;
-  k.tiles_x = cdiv(c.W, 8 * k.S); k.tiles_y = cdiv(c.H, HALO_TH);
-  k.n_blocks = c.Cout_pad / k.block_n;
+  const int S = h.S, bn = h.block_n;
+  k.N = c.N; k.H = c.H; k.W = c.W;
+  k.tiles_x = cdiv(c.W, 8 * S); k.tiles_y = cdiv(c.H, HALO_TH);
+  k.n_blocks = c.Cout_pad / bn;
   k.ntiles = k.tiles_x * k.tiles_y * c.N * k.n_blocks;
-  k.HW = 8 * k.S + k.kw - 1; k.HH = HALO_TH + k.kh - 1;
+  k.HW = 8 * S + k.kw - 1; k.HH = HALO_TH + k.kh - 1;
   k.a_stages = h.a_stages; k.b_stages = h.b_stages; k.a_stage_bytes = h.a_stage_bytes;
-  k.acc_cols = k.S * k.block_n;
-  int cols = 32; while (cols < 2 * k.acc_cols) cols <<= 1;
-  k.tmem_cols = cols;
   k.nsrc = c.nsrc;
   const int es = c.esize == 4 ? 4 : 2;
   k.esize = es; k.chunk = 128 / es; k.round_tf32 = c.round_out_tf32;
@@ -503,17 +283,8 @@ int conv_halo(const ConvTc& c, cudaStream_t s) {
   k.zero_pad_to = c.zero_pad_to > c.Cout ? c.zero_pad_to : c.Cout;
   k.bias = c.bias; k.out = c.out; k.oN = c.oN; k.oH = c.oH; k.oW = c.oW;
   k.res = c.residual; k.rN = c.rN; k.rH = c.rH; k.rW = c.rW;
-  k.tma_out = halo_tma_out(c) ? 1 : 0;
-  k.cw = k.block_n < 64 ? k.block_n : 64;
-  k.stage_out_off = (uint32_t)k.a_stages * (uint32_t)k.a_stage_bytes + (uint32_t)k.b_stages * (uint32_t)k.block_n * 128u;
-  static long long* dbg_buf = nullptr;
-  static int dbg_on = -1;
-  if (dbg_on < 0) dbg_on = env_int("DFVO_HALO_DBG", 0);
-  if (dbg_on && !dbg_buf) { cudaMalloc(&dbg_buf, 8 * sizeof(long long)); }
-  k.dbg = dbg_on ? dbg_buf : nullptr;
-  if (dbg_on) cudaMemsetAsync(dbg_buf, 0, 8 * sizeof(long long), s);
 
-  CUtensorMap tmA[3], tmB, tmO;
+  CUtensorMap tmA[3], tmB;
   for (int i = 0; i < 3; ++i) {
     const ConvTcSource& src = c.src[i < c.nsrc ? i : 0];
     const int inW = c.inW > 0 ? c.inW : c.W, inH = c.inH > 0 ? c.inH : c.H;
@@ -526,58 +297,21 @@ int conv_halo(const ConvTc& c, cudaStream_t s) {
   {
     unsigned long long dims[3] = {(unsigned long long)ktot, (unsigned long long)c.Cout_pad, (unsigned long long)c.ntaps};
     unsigned long long str[2] = {(unsigned long long)ktot * es, (unsigned long long)ktot * es * (unsigned long long)c.Cout_pad};
-    unsigned box[3] = {(unsigned)k.chunk, (unsigned)k.block_n, 1};
+    unsigned box[3] = {(unsigned)k.chunk, (unsigned)bn, 1};
     int rc = tc_encode_map(&tmB, c.w, 3, dims, str, box, es);
     if (rc) return rc;
-  }
-  if (k.tma_out) {
-    // store view: channels [0, max(Cout, zero_pad_to)) of the output slot; boxes are clipped there and at the image border
-    unsigned long long dims[4] = {(unsigned long long)k.zero_pad_to, (unsigned long long)c.W, (unsigned long long)c.H, (unsigned long long)c.N};
-    unsigned long long str[3] = {(unsigned long long)c.oW * 2, (unsigned long long)c.oH * 2, (unsigned long long)c.oN * 2};
-    unsigned box[4] = {(unsigned)k.cw, 8, HALO_TH, 1};
-    int rc = tc_encode_map(&tmO, c.out, 4, dims, str, box, 2, k.cw * 2);
-    if (rc) return rc;
-  } else {
-    tmO = tmB;
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<4, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
   }
   const int grid = k.ntiles < tc_num_sms() ? k.ntiles : tc_num_sms();
   ++g_launch_count;
   TcProf pr;
   const bool prof = tc_prof_begin(s, &pr);
-  cudaLaunchConfig_t cfg; cudaLaunchAttribute attr;
-  tc_launch_config(&cfg, &attr, grid, HALO_THREADS, h.smem, s);
-  if (es == 2) {
-    if (k.S == 1) DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<1, 0>, tmA[0], tmA[1], tmA[2], tmB, tmO, k));
-    else if (k.S == 2) DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<2, 0>, tmA[0], tmA[1], tmA[2], tmB, tmO, k));
-    else DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<4, 0>, tmA[0], tmA[1], tmA[2], tmB, tmO, k));
-  } else {
-    if (k.S == 1) DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<1, 1>, tmA[0], tmA[1], tmA[2], tmB, tmO, k));
-    else if (k.S == 2) DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<2, 1>, tmA[0], tmA[1], tmA[2], tmB, tmO, k));
-    else DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<4, 1>, tmA[0], tmA[1], tmA[2], tmB, tmO, k));
-  }
-  if (dbg_on) {
-    long long t[8];
-    cudaStreamSynchronize(s);
-    cudaMemcpy(t, dbg_buf, sizeof(t), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "halo_dbg N%d %dx%d k%dx%d cin%d cout%d bn%d S%d tiles%d grid%d tma%d | setup %.2f pdl %.2f firstA %.2f acc %.2f store1 %.2f last %.2f us\n",
-            c.N, c.H, c.W, k.kh, k.kw, ktot, c.Cout, k.block_n, k.S, k.ntiles, grid, k.tma_out, (t[1] - t[0]) * 1e-3, (t[2] - t[0]) * 1e-3,
-            (t[3] - t[0]) * 1e-3, (t[4] - t[0]) * 1e-3, (t[5] - t[0]) * 1e-3, ((t[6] ? t[6] : t[5]) - t[0]) * 1e-3);
-  }
+  const int rc = es == 4 ? launch_halo_t<1>(S, bn, tmA, tmB, k, grid, h.smem, s) : launch_halo_t<0>(S, bn, tmA, tmB, k, grid, h.smem, s);
+  if (rc) return rc;
   if (prof) {
     char d[256];
-    snprintf(d, sizeof(d), "halo%s N%d %dx%d k%dx%d src[%d,%d,%d] cout%d/%d bn%d S%d stages%d/%d grid%d tiles%d tma%d gflop %.3f", es == 4 ? "-tf32" : "", c.N, c.H, c.W,
-             k.kh, k.kw, c.src[0].C, c.nsrc > 1 ? c.src[1].C : 0, c.nsrc > 2 ? c.src[2].C : 0, c.Cout, c.Cout_pad, k.block_n,
-             k.S, k.a_stages, k.b_stages, grid, k.ntiles, k.tma_out, c.flops * 1e-9);
+    snprintf(d, sizeof(d), "halo%s N%d %dx%d k%dx%d src[%d,%d,%d] cout%d/%d bn%d S%d stages%d/%d grid%d tiles%d gflop %.3f", es == 4 ? "-tf32" : "", c.N, c.H, c.W,
+             k.kh, k.kw, c.src[0].C, c.nsrc > 1 ? c.src[1].C : 0, c.nsrc > 2 ? c.src[2].C : 0, c.Cout, c.Cout_pad, bn,
+             S, k.a_stages, k.b_stages, grid, k.ntiles, c.flops * 1e-9);
     tc_prof_end(s, pr, c.flops, d);
   }
   DFVO_CHECK_LAUNCH();

@@ -1,15 +1,15 @@
-// tcgen05 implicit-GEMM convolution for sm_100a (stride 1, arbitrary tap set, up to 3 virtually
-// concatenated NHWC bf16 sources, fused bias + activation + residual epilogue).
+// wgmma implicit-GEMM convolution for sm_90a (stride 1 or 2, arbitrary tap set, up to 3 virtually
+// concatenated NHWC bf16 / fp32 sources, fused bias + activation + residual epilogue).
 //
 // GEMM view:  D[128 pixels, BLOCK_N couts] += sum over (tap, source, 64-channel chunk) of
-//             A[128 pixels, 64 ch] * B[BLOCK_N couts, 64 ch]^T        (bf16 x bf16 -> fp32 in TMEM)
+//             A[128 pixels, 64 ch] * B[BLOCK_N couts, 64 ch]^T        (bf16 x bf16 -> fp32 in registers)
 //   * A tile = one TMA 4-D box {64 ch, tw, th, 1} of the NHWC source at pixel offset (dx,dy) of the
 //     tap: the box lands in shared memory as 128 rows x 128 B, K-major, 128-B swizzled -- exactly
-//     the canonical UMMA operand layout, so there is no im2col pass; out-of-image rows/columns
+//     the canonical wgmma operand layout, so there is no im2col pass; out-of-image rows/columns
 //     (the convolution's zero padding) and channels beyond the source's C are zero-filled by TMA.
 //   * B tile = TMA 3-D box {64 k, BLOCK_N, 1 tap} of the packed weights [tap][Cout_pad][Ktot].
-//   * warp 0 = TMA producer, warp 1 = MMA issuer (single thread issues tcgen05.mma, accumulators
-//     double-buffered in TMEM), warps 2-9 = epilogue (tcgen05.ld -> bias/act/residual -> global).
+//   * warp 0 = TMA producer (warps 1-3 idle); warpgroups 1 and 2 = consumers: each issues wgmma for
+//     64 of the 128 pixel rows (accumulators in registers) and runs the bias/act/residual epilogue.
 //   * persistent CTAs, static round-robin tile schedule, mbarrier full/empty smem ring.
 // Restates torch.nn.Conv2d(stride=1) + LeakyReLU/ELU/ReLU as used at lite_flow_net.py:98-240 and
 // depth_decoder.py / torchvision BasicBlock (BN folded by the weight packer).
@@ -47,7 +47,7 @@ struct ConvTcK {
   int8_t dy[49], dx[49];        // stride 1: input offsets; stride 2: offsets in units of double-pixels (floor((k-pad)/2))
   int8_t py[49], px[49];        // stride 2: pixel phase of the tap inside the 2x2 cell
   int stride, src_pitch;        // src_pitch (elements) = channel offset of the odd pixel inside a double-pixel
-  int block_n, stages, acc_stride, tmem_cols;
+  int block_n, stages;
   int Cout, Cout_pad, act, out_f32, zero_pad_to;
   int chunk, esize, round_tf32;   // channels per 128-byte operand row (64 bf16 / 32 tf32), operand element size
   const float* bias;
@@ -59,10 +59,10 @@ struct ConvTcK {
 // =============================================================================================
 //                                       device side
 // =============================================================================================
-#define TC_THREADS 320
+#define TC_THREADS 384
 #define TC_A_BYTES 16384
 
-template <int TF32>
+template <int BN, int TF32>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
           const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB,
@@ -72,15 +72,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B needs 1024-B alignment
   uint8_t* base_ptr = smem_raw + (base - raw);
-  const uint32_t stage_bytes = TC_A_BYTES + (uint32_t)p.block_n * 128u;
+  const uint32_t stage_bytes = TC_A_BYTES + (uint32_t)BN * 128u;
   const uint32_t bar_base = base + (uint32_t)p.stages * stage_bytes;    // 8-byte aligned
-  // barrier layout: full[stages], empty[stages], tmem_full[2], tmem_empty[2]
+  // barrier layout: full[stages], empty[stages]
   auto full_bar = [&](int s) { return bar_base + 8u * (uint32_t)s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (uint32_t)(p.stages + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (uint32_t)(2 * p.stages + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (uint32_t)(2 * p.stages + 2 + a); };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(base_ptr + (size_t)p.stages * stage_bytes + 8u * (2 * p.stages + 4));
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 4);
+  float* bias_s = reinterpret_cast<float*>(base_ptr + (size_t)p.stages * stage_bytes + 8u * (2 * p.stages) + 64);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -88,22 +85,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA0); prefetch_tmap(&tmB);
-    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 8); }
+    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                                  // from here on: activations of the previous kernel / our output buffers
-
-  int chunks_total = 0;
-  for (int s = 0; s < p.nsrc; ++s) chunks_total += (p.srcC[s] + p.chunk - 1) / p.chunk;
 
   if (warp == 0) {
     // ===================================== TMA producer =====================================
@@ -128,7 +114,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
                 tma_load_5d(sa, tm, full_bar(stage), c0 + p.px[tap] * p.src_pitch, x0 + p.dx[tap], p.py[tap], y0 + p.dy[tap], n);
               else
                 tma_load_4d(sa, tm, full_bar(stage), c0, x0 + p.dx[tap], y0 + p.dy[tap], n);
-              tma_load_3d(sa + TC_A_BYTES, &tmB, full_bar(stage), kofs + c0, nb * p.block_n, tap);
+              tma_load_3d(sa + TC_A_BYTES, &tmB, full_bar(stage), kofs + c0, nb * BN, tap);
             }
             __syncwarp();
             if (++stage == p.stages) { stage = 0; phase ^= 1u; }
@@ -137,112 +123,63 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =========================================
-    const uint32_t idesc = tc_idesc(TF32, p.block_n);
-    const uint32_t d_hi = (1024u >> 4) | (1u << 14) | (2u << 29);      // SBO 1024 B, version 1, SWIZZLE_128B
+  } else if (warp >= 4) {
+    // ============================ two consumer warpgroups: MMA + epilogue ============================
+    // warpgroup wg owns rows [64 wg, 64 wg + 64) of the 128-pixel tile: its A operand starts 64 rows = 8 KB into the A box.
+    const int ct = threadIdx.x - 128, wg = ct >> 7, wq = (ct >> 5) & 3;
+    const bool leader = (ct & 127) == 0;
+    for (int i = ct; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = p.round_tf32; ep.out = p.out; ep.res = p.res;
     int stage = 0; uint32_t phase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
+    float acc[BN / 2];
     for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * p.acc_stride);
       uint32_t fresh = 0;
+      int pend = -1;
       for (int tap = 0; tap < p.ntaps; ++tap) {
         for (int s = 0; s < p.nsrc; ++s) {
           for (int c0 = 0; c0 < p.srcC[s]; c0 += p.chunk) {
             mbar_wait(full_bar(stage), phase);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint32_t sa = base + (uint32_t)stage * stage_bytes;
-              const uint32_t a_lo = ((sa >> 4) & 0x3FFFu) | (1u << 16), b_lo = (((sa + TC_A_BYTES) >> 4) & 0x3FFFu) | (1u << 16);
-              const int rem = p.srcC[s] - c0;
-              const int nks = ((rem >= p.chunk ? p.chunk : rem) * p.esize) >> 5;       // 32-byte K steps with real channels
-              if (nks == 4) {
-                tc_mma_lohi<TF32>(tmem_d, a_lo, d_hi, b_lo, d_hi, idesc, fresh);
-                tc_mma_lohi<TF32>(tmem_d, a_lo + 2u, d_hi, b_lo + 2u, d_hi, idesc, 1u);   // +32 B inside the 128-B swizzle atom
-                tc_mma_lohi<TF32>(tmem_d, a_lo + 4u, d_hi, b_lo + 4u, d_hi, idesc, 1u);
-                tc_mma_lohi<TF32>(tmem_d, a_lo + 6u, d_hi, b_lo + 6u, d_hi, idesc, 1u);
-              } else {
-                for (int ks = 0; ks < nks; ++ks)
-                  tc_mma_lohi<TF32>(tmem_d, a_lo + 2u * ks, d_hi, b_lo + 2u * ks, d_hi, idesc, ks == 0 ? fresh : 1u);
-              }
-              tc_commit(empty_bar(stage));
+            wgmma_fence();
+            const uint32_t sa = base + (uint32_t)stage * stage_bytes;
+            const int rem = p.srcC[s] - c0;
+            const int nks = ((rem >= p.chunk ? p.chunk : rem) * p.esize) >> 5;       // 32-byte K steps with real channels
+            float (&acc1)[1][BN / 2] = reinterpret_cast<float (&)[1][BN / 2]>(acc);
+            const uint32_t at = sa + (uint32_t)wg * 8192u, bt = sa + TC_A_BYTES;   // the same K-step walk as one halo tap, S = 1
+            switch (nks) {
+              case 4: halo_tap_mma<1, BN, TF32, 4>(acc1, at, bt, 1024u, fresh); break;
+              case 3: halo_tap_mma<1, BN, TF32, 3>(acc1, at, bt, 1024u, fresh); break;
+              case 2: halo_tap_mma<1, BN, TF32, 2>(acc1, at, bt, 1024u, fresh); break;
+              default: halo_tap_mma<1, BN, TF32, 1>(acc1, at, bt, 1024u, fresh); break;
             }
-            __syncwarp();
+            wgmma_commit();
+            wgmma_wait<1>();                                                          // the previous stage's MMAs are done
+            if (pend >= 0 && leader) mbar_arrive(empty_bar(pend));
+            pend = stage;
             fresh = 1u;
             if (++stage == p.stages) { stage = 0; phase ^= 1u; }
           }
         }
       }
-      if (elect_one()) tc_commit(tfull_bar(acc));
-      __syncwarp();
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
-  } else {
-    // ===================================== epilogue warps ====================================
-    // 8 warps: TMEM lane quadrant = warp % 4 (hardware rule), two warps per quadrant split the columns.
-    const int ew = warp - 2;
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int nchunks = p.block_n >> 4;
-    const int ch_begin = (ew < 4) ? 0 : ((nchunks + 1) >> 1);
-    const int ch_end = (ew < 4) ? ((nchunks + 1) >> 1) : nchunks;
-    // bias staging belongs to the epilogue warps alone (they idle until the first accumulator is ready anyway), so the
-    // producers and the MMA warp start on the barrier-init sync instead of waiting for a global load: ~1 us off the
-    // critical path of each of the ~115 launches per frame.
-    for (int i = threadIdx.x - 64; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float4* bias4 = reinterpret_cast<const float4*>(bias_s);
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+      wgmma_wait<0>();
+      if (leader) mbar_arrive(empty_bar(pend));
+
       int t = tile;
       const int tx = t % p.tiles_x; t /= p.tiles_x;
       const int ty = t % p.tiles_y; t /= p.tiles_y;
       const int n = t % p.N; const int nb = t / p.N;
-      const int x = tx * p.tw + (row % p.tw), y = ty * p.th + (row / p.tw);
-      const bool inb = x < p.W && y < p.H;
-      const int cbase = nb * p.block_n;
-      const long long opix = n * p.oN + y * p.oH + x * p.oW;
-      const long long rpix = n * p.rN + y * p.rH + x * p.rW;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.acc_stride);
-
-      TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = p.round_tf32; ep.out = p.out; ep.res = p.res;
-      // lean path (tc_ptx.cuh::tc_epilogue16_fast): bf16 output, no residual, LeakyReLU / ReLU / identity, aligned pixels
-      const bool fast_launch = !p.out_f32 && p.res == nullptr && p.act <= ACT_RELU && (reinterpret_cast<uintptr_t>(p.out) & 15u) == 0 &&
-                               (p.oW & 7) == 0 && (p.oH & 7) == 0 && (p.oN & 7) == 0;
-      const float slope = p.act == ACT_LEAKY ? 0.1f : (p.act == ACT_RELU ? 0.f : 1.f);
-      auto process = [&](const uint32_t* v, int col) {
-        const int c = cbase + col;
-        if (fast_launch && c + 16 <= p.Cout) tc_epilogue16_fast(v, bias_s + c, slope, reinterpret_cast<__nv_bfloat16*>(p.out) + opix + c, inb);
-        else if (inb && c < p.zero_pad_to) tc_epilogue16_call(ep, v, bias4, c, opix, rpix);
-      };
-
-      for (int ch = ch_begin; ch < ch_end; ch += 2) {
-        uint32_t v0[16], v1[16];
-        const bool two = ch + 1 < ch_end;
-        __syncwarp();                              // tcgen05.ld is .sync.aligned: reconverge first
-        tc_ld16_nowait(taddr0 + (uint32_t)(ch * 16), v0);
-        if (two) tc_ld16_nowait(taddr0 + (uint32_t)(ch * 16 + 16), v1);
-        tc_ld_wait16(v0);
-        if (two) tc_ld_wait16(v1);
-        process(v0, ch * 16);
-        if (two) process(v1, ch * 16 + 16);
+      // accumulator pair (4 j + 2 h, +1) = tile row 64 wg + 16 wq + lane / 4 + 8 h, channels nb * BN + 8 j + 2 (lane % 4) + {0, 1}
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+        const int x = tx * p.tw + (row % p.tw), y = ty * p.th + (row / p.tw);
+        if (x >= p.W || y >= p.H) continue;
+        const long long opix = n * p.oN + y * p.oH + x * p.oW, rpix = n * p.rN + y * p.rH + x * p.rW;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+          tc_store2(ep, bias_s, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], nb * BN + 8 * j + 2 * (lane & 3), opix, rpix);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
   }
 }
 
@@ -306,7 +243,7 @@ int tc_num_sms() {
   if (!g_num_sms) {
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }
@@ -325,9 +262,9 @@ static int build_plan(const ConvTc& c, ConvTcPlanImpl* pl) {
   k.N = c.N; k.H = c.H; k.W = c.W;
   conv_tc_tile_shape(c.H, c.W, &k.tw, &k.th);
   k.tiles_x = cdiv(c.W, k.tw); k.tiles_y = cdiv(c.H, k.th);
-  // N tile: whole Cout_pad if <= 256 else 128-wide blocks
-  k.block_n = c.Cout_pad <= 256 ? c.Cout_pad : 128;
-  DFVO_REQUIRE(c.Cout_pad % k.block_n == 0, DFVO_EINVAL, "conv_tc: Cout_pad %d not divisible by block_n %d", c.Cout_pad, k.block_n);
+  // N tile: the widest wgmma shape (256, 128, 64, 32, 16) that divides Cout_pad
+  k.block_n = 256;
+  while (c.Cout_pad % k.block_n) k.block_n >>= 1;
   k.n_blocks = c.Cout_pad / k.block_n;
   k.ntiles = k.tiles_x * k.tiles_y * c.N * k.n_blocks;
   k.nsrc = c.nsrc; k.ntaps = c.ntaps;
@@ -359,11 +296,8 @@ static int build_plan(const ConvTc& c, ConvTcPlanImpl* pl) {
   k.zero_pad_to = c.zero_pad_to > c.Cout ? c.zero_pad_to : c.Cout;
   k.bias = c.bias; k.out = c.out; k.oN = c.oN; k.oH = c.oH; k.oW = c.oW;
   k.res = c.residual; k.rN = c.rN; k.rH = c.rH; k.rW = c.rW;
-  // TMEM: two accumulators of block_n columns
-  int acc_stride = 32; while (acc_stride < k.block_n) acc_stride <<= 1;
-  k.acc_stride = acc_stride; k.tmem_cols = 2 * acc_stride;
   const size_t stage_bytes = TC_A_BYTES + (size_t)k.block_n * 128;
-  const size_t fixed = 1024 /*align slack*/ + 8 * 64 /*barriers*/ + 64 + (size_t)c.Cout_pad * 4;
+  const size_t fixed = 1024 /*align slack*/ + 8 * 64 /*barriers*/ + 64 + (size_t)c.Cout_pad * 4 /*bias*/;
   int stages = (int)((200 * 1024 - fixed) / stage_bytes);
   if (stages > 8) stages = 8;
   DFVO_REQUIRE(stages >= 2, DFVO_EINVAL, "conv_tc: tile does not fit in shared memory");
@@ -450,24 +384,36 @@ int conv_tc(const ConvTc& c, cudaStream_t s) {
   return conv_tc_single(c, s);
 }
 
+template <int BN, int TF32>
+static int launch_tc(const ConvTcPlanImpl& pl, cudaStream_t s) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    DFVO_CUDA(cudaFuncSetAttribute(k_conv_tc<BN, TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  cudaLaunchConfig_t cfg; cudaLaunchAttribute attr;
+  tc_launch_config(&cfg, &attr, pl.grid, TC_THREADS, pl.smem, s);
+  DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<BN, TF32>, pl.tmA[0], pl.tmA[1], pl.tmA[2], pl.tmB, pl.k));
+  return DFVO_OK;
+}
+
 int conv_tc_single(const ConvTc& c, cudaStream_t s) {
   if (conv_halo_supported(c)) return conv_halo(c, s);
   ConvTcPlanImpl pl;
   int rc = build_plan(c, &pl);
   if (rc) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_tc<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
   ++g_launch_count;
   TcProf pr;
   const bool prof = tc_prof_begin(s, &pr);
-  cudaLaunchConfig_t cfg; cudaLaunchAttribute attr;
-  tc_launch_config(&cfg, &attr, pl.grid, TC_THREADS, pl.smem, s);
-  if (pl.k.esize == 4) DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<1>, pl.tmA[0], pl.tmA[1], pl.tmA[2], pl.tmB, pl.k));
-  else DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<0>, pl.tmA[0], pl.tmA[1], pl.tmA[2], pl.tmB, pl.k));
+  const int tf32 = pl.k.esize == 4;
+  switch (pl.k.block_n) {
+    case 256: rc = tf32 ? launch_tc<256, 1>(pl, s) : launch_tc<256, 0>(pl, s); break;
+    case 128: rc = tf32 ? launch_tc<128, 1>(pl, s) : launch_tc<128, 0>(pl, s); break;
+    case 64: rc = tf32 ? launch_tc<64, 1>(pl, s) : launch_tc<64, 0>(pl, s); break;
+    case 32: rc = tf32 ? launch_tc<32, 1>(pl, s) : launch_tc<32, 0>(pl, s); break;
+    default: rc = tf32 ? launch_tc<16, 1>(pl, s) : launch_tc<16, 0>(pl, s); break;
+  }
+  if (rc) return rc;
   if (prof) {
     char d[256];
     snprintf(d, sizeof(d), "tap  N%d %dx%d s%d taps%d src[%d,%d,%d] cout%d/%d bn%d tile%dx%d stages%d grid%d tiles%d gflop %.3f", c.N, c.H, c.W,

@@ -8,8 +8,8 @@
 // with the 22 (-> 24) second-map pixels of patch row (y + dy) are a [16 x C] x [C x 24] GEMM on mma.sync.m16n8k16 (bf16, fp32
 // accumulate); the 7 wanted displacements are the diagonal band dx = column - pixel of the [16 x 24] result, and in the mma.sync
 // accumulator layout every register has a FIXED (row, column), so the band is picked with compile-time-known predicates.
-// (tcgen05 keeps accumulators in TMEM with lane = row addressing and a warp-uniform column offset, so a per-row column shift --
-// the band -- cannot be read back; the legacy warp-level MMA is the right tensor-core path for a banded product.)  The tensor
+// (the warp-level MMA's fixed fragment layout is what lets the band be selected in registers; a warpgroup MMA would read the
+// 64-row operand once per displacement row for no gain at this size.)  The tensor
 // cores do 24/7 = 3.4x the useful FLOPs, which is irrelevant at 1.2 GFLOP per launch; what matters is that a pixel of the second map
 // is read from shared memory 7 times (once per dy) instead of 49 times, and no scalar FMA is issued at all.
 // Fusions: the Backward warp is evaluated while staging the patch (no warped copy of the feature map in HBM -- and at the stride-2

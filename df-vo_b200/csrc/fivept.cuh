@@ -410,7 +410,9 @@ DFVO_HD bool candidate_from_root(double zr, double zi, const double* c, int n, c
 }
 
 // Full solve.  x1, x2: 5 normalised points each ([5][2]).  E_out: up to 10 row-major 3x3 (x2^T E x1 = 0).
-DFVO_HD int solve(const double* x1, const double* x2, double* E_out) {
+// Kept out of line: inlined into a kernel body, nvcc 12.9's optimiser for sm_90a produces wrong candidates for most
+// samples (tests/test_gpu_depth_pose.py::test_five_point_vs_cv2; -G builds and the out-of-line call are correct).
+static DFVO_HD_NOINLINE int solve(const double* x1, const double* x2, double* E_out) {
   double basis[4][9];
   if (!null_space(x1, x2, basis)) return 0;
   double M[10][20], M0[10][20];

@@ -79,7 +79,7 @@ int resize_bilinear_f32(Ten<const float> in, Ten<float> out, int align_corners, 
 // ---------------------------------------------------------------------------------------------
 // Row-unroll of the 3-channel input for the 7x7 stem (lite_flow_net.py:39-42): out[n,y,x, dx*3+c] =
 // img[n, y, x+dx-3, c] (zero outside), channels 21..31 zero.  The 7x7x3 convolution then is a 7x1
-// convolution over 32 channels, which the tcgen05 kernel can run (its K granularity is 16 channels).
+// convolution over 32 channels, which the wgmma kernel can run (its K granularity is 16 channels).
 // ---------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void k_im2row7(Ten<const float> img, Ten<T> out) {
@@ -636,17 +636,15 @@ k_flow_head(Ten<const bf16> in, const float* __restrict__ w, float b0, float b1,
 #ifndef DFVO_HOSTSIM
 // Register-blocked variant for the device: a thread owns EIGHT output rows of one column, so an input pixel chunk is read from
 // shared memory once per kx and feeds up to 7 x 8 (ky, output row) pairs, and a weight vector once per tap for eight outputs; the
-// two output channels share one packed fma.rn.f32x2 (the pair (w[c][0], w[c][1]) is one 64-bit shared-memory word).  The first
-// kernel above issues 20 LDS.128 per 64 FFMA (shared-memory bound: ncu, 77 us for the 7x7 head at 2x176x608); this one
-// ~0.2 LDS per packed FMA.  Patch layout: [channel chunk q][row][pixel] x 16 B, so the lanes of a warp (consecutive pixels) read
+// weights of the two output channels (w[c][0], w[c][1]) are adjacent in shared memory, so one 128-bit load feeds both channels'
+// FMAs.  The first kernel above issues 20 LDS.128 per 64 FFMA (shared-memory bound); this one ~0.1 LDS per FMA.  Patch layout: [channel chunk q][row][pixel] x 16 B, so the lanes of a warp (consecutive pixels) read
 // consecutive 16-byte words: conflict-free.  Block = 4 warps = 32 columns x 32 rows of outputs.
 #define FH8_TW 32
 #define FH8_RPT 8
 #define FH8_WY 4
-__device__ __forceinline__ void fh_ffma2(unsigned long long& acc, float f, unsigned long long w) {
-  unsigned long long ff;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(ff) : "f"(f));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(ff), "l"(w));
+__device__ __forceinline__ void fh_ffma2(float2& acc, float f, float w0, float w1) {
+  acc.x = fmaf(f, w0, acc.x);
+  acc.y = fmaf(f, w1, acc.y);
 }
 template <int K>
 __global__ void __launch_bounds__(32 * FH8_WY, 2)
@@ -667,9 +665,9 @@ k_flow_head8(Ten<const bf16> in, const float* __restrict__ w, float b0, float b1
     patch[(q * PH + py) * PW + px] = v;
   }
   __syncthreads();
-  unsigned long long acc[FH8_RPT];
+  float2 acc[FH8_RPT];
 #pragma unroll
-  for (int r = 0; r < FH8_RPT; ++r) acc[r] = 0ull;
+  for (int r = 0; r < FH8_RPT; ++r) acc[r] = make_float2(0.f, 0.f);
 #pragma unroll 1
   for (int kx = 0; kx < K; ++kx) {
 #pragma unroll 1
@@ -687,15 +685,15 @@ k_flow_head8(Ten<const bf16> in, const float* __restrict__ w, float b0, float b1
         }
 #pragma unroll
         for (int ky = 0; ky < K; ++ky) {
-          // channels q*8 + half*4 + {0..3}: (c,0) (c,1) pairs = 4 x 64-bit words = 2 x 128-bit loads (broadcast)
-          const ulonglong2* wp = reinterpret_cast<const ulonglong2*>(ws + (ky * K + kx) * 64 + (q * 8 + half * 4) * 2);
-          const ulonglong2 w01 = wp[0], w23 = wp[1];
+          // channels q*8 + half*4 + {0..3}: (c,0) (c,1) pairs = 8 floats = 2 x 128-bit loads (broadcast)
+          const float4* wp = reinterpret_cast<const float4*>(ws + (ky * K + kx) * 64 + (q * 8 + half * 4) * 2);
+          const float4 w01 = wp[0], w23 = wp[1];
 #pragma unroll
           for (int r = 0; r < FH8_RPT; ++r) {
-            fh_ffma2(acc[r], f[r + ky][0], w01.x);
-            fh_ffma2(acc[r], f[r + ky][1], w01.y);
-            fh_ffma2(acc[r], f[r + ky][2], w23.x);
-            fh_ffma2(acc[r], f[r + ky][3], w23.y);
+            fh_ffma2(acc[r], f[r + ky][0], w01.x, w01.y);
+            fh_ffma2(acc[r], f[r + ky][1], w01.z, w01.w);
+            fh_ffma2(acc[r], f[r + ky][2], w23.x, w23.y);
+            fh_ffma2(acc[r], f[r + ky][3], w23.z, w23.w);
           }
         }
       }
@@ -707,8 +705,7 @@ k_flow_head8(Ten<const bf16> in, const float* __restrict__ w, float b0, float b1
   for (int r = 0; r < FH8_RPT; ++r) {
     const int oy = y0 + wy * FH8_RPT + r;
     if (oy >= out.H) break;
-    float a0, a1;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(acc[r]));
+    const float a0 = acc[r].x, a1 = acc[r].y;
     float r0 = 0.f, r1 = 0.f;
     if (has_res) { const float* rr = res.at(n, oy, ox); r0 = rr[0]; r1 = rr[1]; }
     float* o = out.at(n, oy, ox);

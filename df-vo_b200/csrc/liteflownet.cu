@@ -9,7 +9,7 @@
 //   * activations are NHWC; concatenations are channel slots of one buffer that producers write into
 //     directly (no torch.cat copies); small channel groups are zero-padded to 16;
 //   * T = float: every conv on the CUDA-core kernel (parity mode);  T = bf16: stride-1 convs with
-//     >=16 input channels on the tcgen05 kernel, the rest on the CUDA-core kernel.
+//     >=16 input channels on the wgmma kernel, the rest on the CUDA-core kernel.
 #include "liteflownet.h"
 
 #include <stdlib.h>
@@ -48,7 +48,7 @@ template <> struct IsBf16<bf16> { enum { v = 1 }; };
 template <typename T>
 struct LfnImpl : public LiteFlowNetBase {
   Arena arena;
-  bool tf32 = false;          // T = float only: convs on tcgen05 kind::tf32 (DFVO_PREC_TF32) instead of the CUDA-core kernel
+  bool tf32 = false;          // T = float only: convs on wgmma tf32 (DFVO_PREC_TF32) instead of the CUDA-core kernel
   int H0 = 0, W0 = 0, th = 0, tw = 0, B = 0, P = 0;
   int lh[7], lw[7];
   // weights
@@ -251,7 +251,7 @@ struct LfnImpl : public LiteFlowNetBase {
   int features(cudaStream_t s) {
     for (int L = 2; L <= 6; ++L) TRY(resize_bilinear_f32(cfview(img[L - 1], L - 1, 3, 4), fview(img[L], L, 4, 4), 0, s));
     Ten<const T> none; memset(&none, 0, sizeof(none));
-    // level 1: 7x7 3->32.  bf16: row-unroll + tcgen05 7x1 conv;  fp32: CUDA-core kernel on the float image
+    // level 1: 7x7 3->32.  bf16: row-unroll + wgmma 7x1 conv;  fp32: CUDA-core kernel on the float image
     if (IsBf16<T>::v && stem_window) {
       Ten<T> pad = make_ten<T>(imgpad, B, lh[1], lw[1] + 8, 8, 8);
       TRY(pad_image8<T>(cfview(img[1], 1, 3, 4), pad, s));

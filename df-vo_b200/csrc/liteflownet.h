@@ -21,7 +21,7 @@ struct LiteFlowNetBase {
 
 void liteflow_target_size(int h, int w, int* th, int* tw);
 
-// precision: 0 = fp32 everywhere (CUDA-core convs), 1 = bf16 activations + tcgen05 convs
+// precision: 0 = fp32 everywhere (CUDA-core convs), 1 = bf16 activations + wgmma convs
 int liteflownet_create(const WeightStore& ws, int H0, int W0, int pairs, int precision, LiteFlowNetBase** out);
 
 }  // namespace dfvo

@@ -8,7 +8,7 @@
 //
 // Layout/plan: NHWC; every 3x3 decoder conv reads a reflection-padded buffer produced by one fused
 // "nearest-upsample + concat skip + reflect-pad" kernel, so the convs are plain valid convs and run on
-// the tcgen05 kernel (T = bf16) or the CUDA-core kernel (T = float, parity mode; stride-2 / 3-channel /
+// the wgmma kernel (T = bf16) or the CUDA-core kernel (T = float, parity mode; stride-2 / 3-channel /
 // 1-channel layers in both modes).
 #include <stdlib.h>
 #include "monodepth2.h"
@@ -24,7 +24,7 @@ template <> struct IsBf16m<bf16> { enum { v = 1 }; };
 template <typename T>
 struct MonoImpl : public Monodepth2Base {
   Arena arena;
-  bool tf32 = false;          // T = float only: tcgen05 kind::tf32 convs (DFVO_PREC_TF32)
+  bool tf32 = false;          // T = float only: wgmma tf32 convs (DFVO_PREC_TF32)
   int h = 0, w = 0;
   float min_depth = 0.1f, max_depth = 100.f, baseline = 5.4f;
   ConvLayer conv1;

@@ -228,7 +228,7 @@ template int run_conv_multi<float>(const ConvLayer&, const Ten<const float>*, in
 template <>
 int run_conv<float>(const ConvLayer& L, Ten<const float> in, Ten<float> out, int act, Ten<const float> residual,
                     int zero_pad_to, cudaStream_t s) {
-  // tf32 mode: fp32 activations, tcgen05 kind::tf32; stored activations are rounded to tf32 (the next conv's operand)
+  // tf32 mode: fp32 activations, wgmma tf32; stored activations are rounded to tf32 (the next conv's operand)
   if (L.tc && L.tc_esize == 4) return launch_tc<float, float>(L, in, out, act, residual, zero_pad_to, 1, s);
   DFVO_REQUIRE(L.w_direct, DFVO_ESTATE, "conv layer has no fp32 weights");
   // pad channels of fp32 buffers are zero from allocation and never written; nothing to do for zero_pad_to
@@ -258,8 +258,7 @@ int run_conv_f32out<bf16>(const ConvLayer& L, Ten<const bf16> in, Ten<float> out
   if (!L.tc) return conv_direct<bf16, float>(to_direct(L, act), in, out, residual, s);
   // 2-channel flow heads: dedicated CUDA-core kernel; the tensor-core kernel (N padded to 16) serves the other
   // float-output layers (monodepth2's disparity head)
-  // (measured with ncu on B200: the 7x7 head at 176x608x2 takes 77 us on the CUDA-core kernel and 94 us on the tensor-core
-  //  kernel -- 49 taps of N = 16 MMAs are issue / barrier bound -- so the tensor-core route is opt-in: DFVO_HEAD_TC=1)
+  // (49 taps of N = 16 MMAs are issue / barrier bound, so the tensor-core route is opt-in: DFVO_HEAD_TC=1)
   static int head_tc = -1;
   if (head_tc < 0) { const char* e = getenv("DFVO_HEAD_TC"); head_tc = (e && atoi(e) == 1); }
   const bool big = (long long)in.N * in.H * in.W >= 100000;

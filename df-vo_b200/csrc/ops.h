@@ -81,9 +81,9 @@ int conv_direct(const ConvDirect& c, Ten<const TI> in, Ten<TO> out, Ten<const TO
 int flow_head(Ten<const __nv_bfloat16> in, const float* w, float bias0, float bias1, int k, Ten<const float> residual,
               Ten<float> out, cudaStream_t s);
 
-// ---- tcgen05 implicit-GEMM convolution (conv_tc.cu) -------------------------------------------
+// ---- wgmma implicit-GEMM convolution (conv_tc.cu) ---------------------------------------------
 struct ConvTcSource {
-  const void* p;          // NHWC view (channel slice allowed) of bf16 (esize 2) or float (esize 4, kind::tf32) elements
+  const void* p;          // NHWC view (channel slice allowed) of bf16 (esize 2) or float (esize 4, read as tf32) elements
   int C;                  // channels in this source (multiple of 16; zero-padded by the producer)
   long long sN, sH, sW;   // strides in elements
 };
@@ -97,7 +97,7 @@ struct ConvTc {
                           // 5-D tensor map (pitch+C, W/2, 2, H/2, N) -- see conv_tc.cu)
   int ntaps;              // kh*kw
   int8_t dy[49], dx[49];  // tap offsets in INPUT pixels (already include -pad): iy = oy*stride + dy
-  int esize;              // operand element size: 2 = bf16 (tcgen05 kind::f16), 4 = fp32 storage read as tf32 (kind::tf32)
+  int esize;              // operand element size: 2 = bf16, 4 = fp32 storage read as tf32
   int round_out_tf32;     // esize 4: round the stored fp32 activations to tf32 (cvt.rna) so the next conv's operand is unbiased
   const void* w;          // packed [ntaps][Cout_pad][Ktot] (bf16 or tf32-rounded float), Ktot = sum(src[i].C)
   int Cout_pad;           // multiple of 16

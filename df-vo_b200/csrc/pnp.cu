@@ -310,8 +310,8 @@ DFVO_HD bool solve(int n, const double pw[][3], const double uv[][2], double fu,
 //     cv::SVD (it fixes the signs and the basis inside the rank-deficient null space, see ocv_svd); what differs from the
 //     one-thread path is round-off only: the order of the 12 additions inside a dot product, and the rotation (c, s) evaluated with
 //     two reciprocal square roots instead of hypot + 2 divisions + 2 square roots (the dependent FP64 chain that dominates a pair:
-//     measured on B200, a first version that kept the division / sqrt chain and packed two samples per warp was 2.2x SLOWER than
-//     the one-thread kernel -- the two halves diverge on every skipped pair);
+//     a version that keeps the division / sqrt chain and packs two samples per warp is slower than the one-thread kernel --
+//     the two halves diverge on every skipped pair);
 //   * control points / barycentric coordinates / L / rho are recomputed redundantly by every lane (no communication);
 //   * the three beta approximations + Gauss-Newton + absolute orientation run on lanes 0, 1, 2 in parallel; the winner (first
 //     strictly smaller reprojection error, as in the sequential loop) is broadcast.

@@ -252,7 +252,7 @@ int local_bestn(const float* diff, const float* depth_diff, int H, int W, int ro
                 float depth_thre, int N_total, int32_t* idx_out, int32_t* cell_counts, int32_t* status, cudaStream_t s) {
   DFVO_REQUIRE(rows > 0 && cols > 0 && n_best > 0 && rows * cols <= 65535, DFVO_EINVAL, "local_bestn args");
   DFVO_CUDA(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), s));
-  DFVO_LAUNCH(k_count_below, dim3(148), dim3(SEL_THREADS), 0, s, diff, H * W, thre, status + 2);
+  DFVO_LAUNCH(k_count_below, dim3(132), dim3(SEL_THREADS), 0, s, diff, H * W, thre, status + 2);
   DFVO_CHECK_LAUNCH();
   DFVO_LAUNCH(k_local_bestn, dim3(rows * cols), dim3(SEL_THREADS), 0, s, diff, depth_diff, H, W, rows, cols, n_best, thre,
               depth_thre, idx_out, cell_counts);
@@ -366,7 +366,7 @@ int bestn(const float* diff, int H, int W, int N, int32_t* idx_out, void* worksp
   const int nblocks = cdiv(n, BESTN_CHUNK);
   DFVO_LAUNCH(k_bestn_init, dim3(1), dim3(256), 0, s, ws, N);
   for (int pass = 0; pass < 4; ++pass) {
-    DFVO_LAUNCH(k_bestn_hist, dim3(148), dim3(SEL_THREADS), 0, s, diff, n, pass, ws);
+    DFVO_LAUNCH(k_bestn_hist, dim3(132), dim3(SEL_THREADS), 0, s, diff, n, pass, ws);
     DFVO_LAUNCH(k_bestn_pick, dim3(1), dim3(256), 0, s, pass, ws);
   }
   DFVO_LAUNCH(k_bestn_count, dim3(nblocks), dim3(SEL_THREADS), 0, s, diff, n, ws);

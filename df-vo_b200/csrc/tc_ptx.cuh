@@ -1,11 +1,14 @@
-// tcgen05 / TMA / mbarrier PTX wrappers and the fused conv epilogue shared by the two tensor-core convolution
-// kernels (conv_tc.cu: per-tap operand loads, stride 1|2;  conv_halo.cu: halo-resident operand, stride 1).
+// wgmma / TMA / mbarrier PTX wrappers, the fused conv epilogue and the MMA consumer shared by the tensor-core convolution
+// kernels (conv_tc.cu: per-tap operand loads, stride 1|2;  conv_halo.cu / conv_chain.cu: halo-resident operand, stride 1).
 #pragma once
 #include "ops.h"
+#ifndef DFVO_HOSTSIM
+#include "wgmma.cuh"
+#endif
 
 namespace dfvo {
 
-// what the epilogue needs to turn 16 accumulator columns of one output pixel into stored channels
+// what the epilogue needs to turn accumulator columns of one output pixel into stored channels
 struct TcEpi {
   int Cout, zero_pad_to, act, out_f32;
   int round_tf32;          // fp32 output rounded to the tf32 grid (tf32 mode activations)
@@ -51,70 +54,20 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* tmap, uint
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"((uint64_t)tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// ---- TMA store (shared -> global) of one tile box; bulk-group completion tracking
-__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"((uint64_t)tmap), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all but the newest `N` bulk groups have finished READING shared memory (their staging buffers may be overwritten)
+// ---- wgmma (warpgroup MMA) ordering: fence before the first MMA that touches accumulator registers the warpgroup has read or
+// written since its last MMA; commit closes a group of issued MMAs; wait<N> returns once at most N groups are still in flight
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-// all bulk groups are complete (global writes performed)
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// generic-proxy shared-memory writes -> visible to the async proxy (TMA) before the store is issued
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// MMA with the two 64-bit shared-memory descriptors given as (lo, hi) words: the hi words (SBO / version / swizzle) are
-// loop invariants, only the 14-bit start-address field in lo changes between issues
-__device__ __forceinline__ void tc_mma_bf16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-// kind::tf32: fp32 operands in shared memory read as tf32 (upper 19 bits), K = 8 per instruction (32 bytes per row, like bf16's
-// K = 16), fp32 accumulation.  Same descriptors, same 128-byte swizzle.
-__device__ __forceinline__ void tc_mma_tf32_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-template <int TF32>
-__device__ __forceinline__ void tc_mma_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                            uint32_t accumulate) {
-  if (TF32) tc_mma_tf32_lohi(tmem_d, a_lo, a_hi, b_lo, b_hi, idesc, accumulate);
-  else tc_mma_bf16_lohi(tmem_d, a_lo, a_hi, b_lo, b_hi, idesc, accumulate);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = f32 (1 @ bit 4), A / B format @ bits 7 / 10 (kind::f16: bf16 = 1;
-// kind::tf32: tf32 = 2), K-major A and B, N >> 3 @ 17, M >> 4 @ 24
-__device__ __forceinline__ uint32_t tc_idesc(int tf32, int block_n) {
-  const uint32_t fmt = tf32 ? 2u : 1u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(block_n >> 3) << 17) | ((128u >> 4) << 24);
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// K-major, 128-byte-swizzle shared-memory matrix descriptor (sm_90 GMMA layout): start>>4 [0,14) | LBO>>4 [16,30) (unused for
+// swizzled K-major, 1) | SBO>>4 [32,46) = distance of consecutive 8-row groups | base offset [49,52) = 0 | SWIZZLE_128B (1) [62,64).
+// The swizzle XOR is a function of the absolute shared-memory address and the pattern starts at the 1024-B aligned stage base
+// (base offset 0), so a start shifted by whole 128-B rows or by 32 B inside a row addresses exactly the bytes TMA wrote there.
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr, uint32_t sbo_bytes) {
+  const uint32_t lo = ((saddr >> 4) & 0x3FFFu) | (1u << 16);
+  const uint32_t hi = ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 30);
+  return ((uint64_t)hi << 32) | lo;
 }
 __device__ __forceinline__ float tc_round_tf32(float v) {
   uint32_t r;
@@ -125,13 +78,13 @@ __device__ __forceinline__ float tc_round_tf32(float v) {
 // while its predecessor in the stream is still running; it must not touch data the predecessor produces (or overwrite
 // data it reads) before pdl_wait(), which returns once the predecessor grid has completed and flushed.  pdl_trigger()
 // lets the *next* kernel of the stream start its own prologue early.  The convolution kernels run their prologue
-// (barrier init, TMEM allocation, tensor-map prefetch, bias staging: nothing a predecessor writes) before the wait.
+// (barrier init, tensor-map prefetch: nothing a predecessor writes) before the wait.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)tmap) : "memory");
 }
-// one elected lane of a fully active warp (cute::elect_one_sync): ptxas keeps tcgen05 / TMA issues under this
+// one elected lane of a fully active warp (cute::elect_one_sync): ptxas keeps TMA issues under this
 // predicate on the uniform datapath without the per-instruction ELECT loop it emits under `if (lane == 0)`
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -142,227 +95,137 @@ __device__ __forceinline__ bool elect_one() {
       : "+r"(pred));
   return pred != 0;
 }
-// wait for outstanding tcgen05.ld; the registers are in/out operands so no use can be hoisted above it
-__device__ __forceinline__ void tc_ld_wait16(uint32_t* v) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                 "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])
-               :: "memory");
-}
-__device__ __forceinline__ void tc_ld16_nowait(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// K-major, 128-byte-swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
-// start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
-  uint64_t d = (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
 }  // namespace tc
 
-// Slow path of the epilogue (partial channel groups, unaligned pixels, fp32 outputs: the 2-channel heads, the 1-channel
-// disparity head, 9/25/49-channel distance maps).  Deliberately NOT inlined and with rolled loops: the convolution
-// kernels are launched ~115 times per frame, most of them for a few microseconds, and every kilobyte of unrolled
-// epilogue is instruction-cache traffic at each of those launches.
-static __device__ __noinline__ void tc_epilogue16_slow(TcEpi p, float4 f0, float4 f1, float4 f2, float4 f3, int c, long long opix,
-                                                        long long rpix) {
-  const float f[16] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w, f2.x, f2.y, f2.z, f2.w, f3.x, f3.y, f3.z, f3.w};
-  if (!p.out_f32) {
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + opix + c;
-    const __nv_bfloat16* r = p.res ? reinterpret_cast<const __nv_bfloat16*>(p.res) + rpix + c : nullptr;
-#pragma unroll 1
-    for (int j = 0; j < 16; ++j) {
-      if (c + j < p.Cout) {
-        const float val = f[j] + (r ? __bfloat162float(r[j]) : 0.f);
-        o[j] = __float2bfloat16_rn(apply_act(val, p.act));
-      } else if (c + j < p.zero_pad_to) {
-        o[j] = __float2bfloat16_rn(0.f);
-      }
+// bias + optional residual + activation + store of the two adjacent output channels (c, c + 1) of one pixel (c even): the pair a
+// thread holds in the wgmma accumulator fragment.  opix / rpix = element offsets of the pixel; channels in [Cout, zero_pad_to) are
+// written as zeros, channels from zero_pad_to on are not written.
+__device__ __forceinline__ void tc_store2(const TcEpi& p, const float* bias, float a, float b, int c, long long opix, long long rpix) {
+  if (c >= p.zero_pad_to) return;
+  const bool two = c + 1 < p.zero_pad_to;
+  float v[2] = {a, b};
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    if (c + j < p.Cout) {
+      float x = v[j] + bias[c + j];
+      if (p.res) x += p.out_f32 ? reinterpret_cast<const float*>(p.res)[rpix + c + j]
+                                : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.res)[rpix + c + j]);
+      v[j] = apply_act(x, p.act);
+    } else {
+      v[j] = 0.f;
+    }
+  }
+  if (p.out_f32) {
+    if (p.round_tf32) { v[0] = tc::tc_round_tf32(v[0]); v[1] = tc::tc_round_tf32(v[1]); }
+    float* o = reinterpret_cast<float*>(p.out) + opix + c;
+    if (two && (reinterpret_cast<uintptr_t>(o) & 7u) == 0) {
+      *reinterpret_cast<float2*>(o) = make_float2(v[0], v[1]);
+    } else {
+      o[0] = v[0];
+      if (two) o[1] = v[1];
     }
   } else {
-    float* o = reinterpret_cast<float*>(p.out) + opix + c;
-    const float* r = p.res ? reinterpret_cast<const float*>(p.res) + rpix + c : nullptr;
-#pragma unroll 1
-    for (int j = 0; j < 16; ++j) {
-      if (c + j < p.Cout) {
-        const float val = f[j] + (r ? r[j] : 0.f);
-        o[j] = apply_act(val, p.act);
-      } else if (c + j < p.zero_pad_to) {
-        o[j] = 0.f;
-      }
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + opix + c;
+    if (two && (reinterpret_cast<uintptr_t>(o) & 3u) == 0) {
+      *reinterpret_cast<__nv_bfloat162*>(o) = __floats2bfloat162_rn(v[0], v[1]);
+    } else {
+      o[0] = __float2bfloat16_rn(v[0]);
+      if (two) o[1] = __float2bfloat16_rn(v[1]);
     }
   }
 }
 
-// Lean epilogue for the common case (bf16 output, no residual, LeakyReLU / ReLU / identity, all 16 channels real, 16-byte aligned
-// pixel): v = 16 fp32 accumulator words, bias = 16 floats in shared memory.  ncu showed the generic path costing 374 instructions per
-// two chunks (integer divisions, per-chunk alignment / tail / slow-path tests, scalar FADD / FMUL) and the epilogue warps -- two
-// per scheduler -- issue-bound at ~20 %: 7.7 us per 256 x 128 tile against 4.8 us of MMAs.  Here: 8 FADD2 + 8 FMUL2 (packed fp32x2,
-// sm_100) + 16 FMNMX + 8 F2FP + 2 STG.128.
-__device__ __forceinline__ void tc_epilogue16_fast_pack(const uint32_t* v, const float* bias, float slope, uint32_t* w) {
-  const float4* b4 = reinterpret_cast<const float4*>(bias);
-  unsigned long long sl;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(sl) : "f"(slope));
+// An mbarrier-guarded ring of shared-memory slots as one side walks it: slot i, its full / empty barriers, the phase bit.
+struct TcRing {
+  uint32_t base, slot_bytes, full0, empty0;
+  int n, i;
+  uint32_t ph;
+  __device__ __forceinline__ uint32_t slot() const { return base + (uint32_t)i * slot_bytes; }
+  __device__ __forceinline__ uint32_t full() const { return full0 + 8u * (uint32_t)i; }
+  __device__ __forceinline__ uint32_t empty() const { return empty0 + 8u * (uint32_t)i; }
+  __device__ __forceinline__ void next() { if (++i == n) { i = 0; ph ^= 1u; } }
+};
+
+// the MMAs of one tap: S sub-tiles (+8 pixels = +1024 B each) x NKS K steps (+32 B inside the 128-B swizzle atom)
+template <int S, int BN, int TF32, int NKS>
+__device__ __forceinline__ void halo_tap_mma(float (&acc)[S][BN / 2], uint32_t at, uint32_t bt, uint32_t a_sbo, uint32_t fresh) {
+  using namespace tc;
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float4 b = b4[j];
-    unsigned long long a0, a1, b0, b1, x0, x1, y0, y1;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a0) : "r"(v[4 * j]), "r"(v[4 * j + 1]));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(a1) : "r"(v[4 * j + 2]), "r"(v[4 * j + 3]));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b0) : "f"(b.x), "f"(b.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b1) : "f"(b.z), "f"(b.w));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(x0) : "l"(a0), "l"(b0));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(x1) : "l"(a1), "l"(b1));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(y0) : "l"(x0), "l"(sl));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(y1) : "l"(x1), "l"(sl));
-    float xa, xb, xc, xd, ya, yb, yc, yd;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(xa), "=f"(xb) : "l"(x0));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(xc), "=f"(xd) : "l"(x1));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(ya), "=f"(yb) : "l"(y0));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(yc), "=f"(yd) : "l"(y1));
-    __nv_bfloat162 h0 = __floats2bfloat162_rn(fmaxf(xa, ya), fmaxf(xb, yb));
-    __nv_bfloat162 h1 = __floats2bfloat162_rn(fmaxf(xc, yc), fmaxf(xd, yd));
-    w[2 * j] = *reinterpret_cast<uint32_t*>(&h0);
-    w[2 * j + 1] = *reinterpret_cast<uint32_t*>(&h1);
-  }
-}
-__device__ __forceinline__ void tc_epilogue16_fast(const uint32_t* v, const float* bias, float slope, __nv_bfloat16* o, bool valid) {
-  uint32_t w[8];
-  tc_epilogue16_fast_pack(v, bias, slope, w);
-  if (valid) {
-    *reinterpret_cast<uint4*>(o) = make_uint4(w[0], w[1], w[2], w[3]);
-    *reinterpret_cast<uint4*>(o + 8) = make_uint4(w[4], w[5], w[6], w[7]);
-  }
+  for (int sub = 0; sub < S; ++sub)
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks)
+      Wgmma<BN, TF32>::mma(acc[sub], desc_sw128(at + (uint32_t)sub * 1024u + 32u * ks, a_sbo), desc_sw128(bt + 32u * ks, 1024u),
+                           ks == 0 ? fresh : 1u);
 }
 
-// bias + optional residual + activation + store of 16 consecutive output channels [c, c+16) of one pixel.
-// v = 16 fp32 accumulator words (tcgen05.ld), bias4 = shared-memory bias, opix/rpix = element offsets of the pixel.
-// Fast path (bf16 output, full aligned group): two 16-byte stores; LeakyReLU / ReLU / identity are one fmaxf with a
-// per-launch slope (0.1 / 0 / 1), only ELU / sigmoid branch.
-__device__ __forceinline__ void tc_epilogue16(const TcEpi& p, const uint32_t* v, const float4* bias4, int c, long long opix, long long rpix) {
-  float f[16];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float4 b = bias4[(c >> 2) + j];
-    f[4 * j + 0] = __uint_as_float(v[4 * j + 0]) + b.x;
-    f[4 * j + 1] = __uint_as_float(v[4 * j + 1]) + b.y;
-    f[4 * j + 2] = __uint_as_float(v[4 * j + 2]) + b.z;
-    f[4 * j + 3] = __uint_as_float(v[4 * j + 3]) + b.w;
-  }
-  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + opix + c;
-  const __nv_bfloat16* r = p.res ? reinterpret_cast<const __nv_bfloat16*>(p.res) + rpix + c : nullptr;
-  // a group that straddles Cout but lies inside the zero-padded range (49 -> 64, 25 -> 32, 9 -> 16 distance channels) is
-  // still two vector stores: channels >= Cout are written as zeros
-  const int cend = p.Cout > p.zero_pad_to ? p.Cout : p.zero_pad_to;
-  const bool tail = c + 16 > p.Cout;
-  if (p.out_f32 && (c + 16 <= cend)) {
-    // fp32 activations (tf32 mode): four 16-byte stores; pad channels of a straddling group are written as zeros
-    float* of = reinterpret_cast<float*>(p.out) + opix + c;
-    const float* rf = p.res ? reinterpret_cast<const float*>(p.res) + rpix + c : nullptr;
-    if ((reinterpret_cast<uintptr_t>(of) & 15u) == 0 && (!rf || (!tail && (reinterpret_cast<uintptr_t>(rf) & 15u) == 0))) {
-      if (rf) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 rv = *reinterpret_cast<const float4*>(rf + 4 * j);
-          f[4 * j] += rv.x; f[4 * j + 1] += rv.y; f[4 * j + 2] += rv.z; f[4 * j + 3] += rv.w;
+// MMA main loop of one tile of the halo-resident kernels (conv_halo.cu, conv_chain.cu) for one consumer warpgroup: wg 0 / 1 owns
+// pixel rows 0-7 / 8-15 of every 8 x 16 sub-tile (M = 64 each).  Per (source, channel chunk) one A slot holds the HW x HH pixel
+// halo (128 B per pixel, SWIZZLE_128B); tap (ky, kx) reads it through a descriptor whose start is shifted by (ky * HW + kx) pixels
+// and whose SBO is one halo row, so the 8-row groups of the K-major operand are the sub-tile's pixel rows.  One B slot per tap
+// (BN x 128 B of weights) is shared by the S sub-tiles and released once the MMAs of the next tap are issued and its own have
+// completed; the A slot is released at the end of its chunk.  `leader` = one thread of the warpgroup (the empty barriers count
+// one arrival per consumer warpgroup).
+template <int S, int BN, int TF32>
+__device__ __forceinline__ void halo_tile_mma(float (&acc)[S][BN / 2], TcRing& ra, TcRing& rb, int nsrc, const int* srcC, int chunk,
+                                              int esize, int kh, int kw, int HW, int wg, bool leader) {
+  using namespace tc;
+  const uint32_t a_sbo = (uint32_t)HW * 128u;
+  uint32_t fresh = 0;                         // 0 for the first (chunk, tap) of the tile: its ks = 0 MMAs overwrite
+  for (int s = 0; s < nsrc; ++s) {
+    for (int c0 = 0; c0 < srcC[s]; c0 += chunk) {
+      const int rem = srcC[s] - c0;
+      const int nks = ((rem >= chunk ? chunk : rem) * esize) >> 5;        // 32-byte K steps (16 bf16 / 8 tf32) with real channels
+      mbar_wait(ra.full(), ra.ph);
+      const uint32_t a0 = ra.slot() + (uint32_t)wg * 8u * a_sbo;
+      int pend = -1;
+      for (int ky = 0; ky < kh; ++ky) {
+        for (int kx = 0; kx < kw; ++kx) {
+          mbar_wait(rb.full(), rb.ph);
+          wgmma_fence();
+          const uint32_t at = a0 + (uint32_t)(ky * HW + kx) * 128u, bt = rb.slot();
+          switch (nks) {                                                   // compile-time K steps: no wgmma in a run-time loop
+            case 4: halo_tap_mma<S, BN, TF32, 4>(acc, at, bt, a_sbo, fresh); break;
+            case 3: halo_tap_mma<S, BN, TF32, 3>(acc, at, bt, a_sbo, fresh); break;
+            case 2: halo_tap_mma<S, BN, TF32, 2>(acc, at, bt, a_sbo, fresh); break;
+            default: halo_tap_mma<S, BN, TF32, 1>(acc, at, bt, a_sbo, fresh); break;
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (pend >= 0 && leader) mbar_arrive(rb.empty0 + 8u * (uint32_t)pend);
+          pend = rb.i;
+          rb.next();
+          fresh = 1u;
         }
       }
-      if (p.act <= ACT_RELU) {
-        const float slope = p.act == ACT_LEAKY ? 0.1f : (p.act == ACT_RELU ? 0.f : 1.f);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], slope * f[j]);
-      } else if (p.act == ACT_ELU) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = f[j] > 0.f ? f[j] : expm1f(f[j]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = 1.f / (1.f + expf(-f[j]));
-      }
-      if (tail) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = (c + j < p.Cout) ? f[j] : 0.f;
-      }
-      if (p.round_tf32) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = tc::tc_round_tf32(f[j]);
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) *reinterpret_cast<float4*>(of + 4 * j) = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-      return;
+      wgmma_wait<0>();
+      if (leader) { mbar_arrive(rb.empty0 + 8u * (uint32_t)pend); mbar_arrive(ra.empty()); }
+      ra.next();
     }
   }
-  const bool full = !p.out_f32 && (c + 16 <= cend) && ((reinterpret_cast<uintptr_t>(o) & 15u) == 0) &&
-                    (!r || (!tail && (reinterpret_cast<uintptr_t>(r) & 15u) == 0));
-  if (!full) {
-    tc_epilogue16_slow(p, make_float4(f[0], f[1], f[2], f[3]), make_float4(f[4], f[5], f[6], f[7]), make_float4(f[8], f[9], f[10], f[11]),
-                       make_float4(f[12], f[13], f[14], f[15]), c, opix, rpix);
-    return;
-  }
-  if (r) {
-    const uint4 r0 = *reinterpret_cast<const uint4*>(r), r1 = *reinterpret_cast<const uint4*>(r + 8);
-    const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+}
+
+// Epilogue of one halo tile for one consumer warpgroup: the thread's accumulator pairs are pixels (x0 + 8 sub + lane / 4,
+// y0 + 8 wg + 2 warp + h), channels cbase + 8 j + 2 (lane % 4) + {0, 1}.
+template <int S, int BN>
+__device__ __forceinline__ void halo_tile_store(const float (&acc)[S][BN / 2], const TcEpi& ep, const float* bias_s, int cbase, int n,
+                                                int x0, int y0, int W, int H, long long oN, long long oH, long long oW, long long rN,
+                                                long long rH, long long rW, int wg, int warp_in_wg, int lane) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      f[2 * j] += __uint_as_float(rw[j] << 16);
-      f[2 * j + 1] += __uint_as_float(rw[j] & 0xffff0000u);
+  for (int h = 0; h < 2; ++h) {
+    const int y = y0 + 8 * wg + 2 * warp_in_wg + h;
+    if (y >= H) continue;
+#pragma unroll
+    for (int sub = 0; sub < S; ++sub) {
+      const int x = x0 + 8 * sub + (lane >> 2);
+      if (x >= W) continue;
+      const long long opix = n * oN + y * oH + x * oW, rpix = n * rN + y * rH + x * rW;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+        tc_store2(ep, bias_s, acc[sub][4 * j + 2 * h], acc[sub][4 * j + 2 * h + 1], cbase + 8 * j + 2 * (lane & 3), opix, rpix);
     }
   }
-  if (p.act <= ACT_RELU) {
-    const float slope = p.act == ACT_LEAKY ? 0.1f : (p.act == ACT_RELU ? 0.f : 1.f);      // max(f, f) = f for ACT_NONE
-#pragma unroll
-    for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], slope * f[j]);
-  } else if (p.act == ACT_ELU) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) f[j] = f[j] > 0.f ? f[j] : expm1f(f[j]);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) f[j] = 1.f / (1.f + expf(-f[j]));
-  }
-  if (tail) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) f[j] = (c + j < p.Cout) ? f[j] : 0.f;
-  }
-  uint32_t w[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-    w[j] = *reinterpret_cast<uint32_t*>(&h);
-  }
-  *reinterpret_cast<uint4*>(o) = make_uint4(w[0], w[1], w[2], w[3]);
-  *reinterpret_cast<uint4*>(o + 8) = make_uint4(w[4], w[5], w[6], w[7]);
 }
-// Out-of-line instance of the general epilogue for the conv kernels' rare chunks (residual / ELU / sigmoid / fp32 output / channel
-// tails): one copy of the ~15 KB of unrolled activation code per kernel instead of one per call site (the kernels were 128 KB of
-// SASS; ncu showed `no_instruction` stalls in the epilogue warps).  The accumulator words travel by value (registers).
-struct TcAcc16 { uint32_t v[16]; };
-static __device__ __noinline__ void tc_epilogue16_general(TcEpi p, TcAcc16 a, const float4* bias4, int c, long long opix, long long rpix) {
-  tc_epilogue16(p, a.v, bias4, c, opix, rpix);
-}
-__device__ __forceinline__ void tc_epilogue16_call(const TcEpi& p, const uint32_t* v, const float4* bias4, int c, long long opix, long long rpix) {
-  TcAcc16 a;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) a.v[j] = v[j];
-  tc_epilogue16_general(p, a, bias4, c, opix, rpix);
-}
+
 #endif  // !DFVO_HOSTSIM
 
 // internal: the halo-resident kernel (conv_halo.cu); conv_tc() dispatches to it for stride-1 rectangular tap sets

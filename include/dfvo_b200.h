@@ -1,4 +1,4 @@
-/* dfvo_b200 -- C ABI of the B200-native DF-VO tracking hot path (libdfvo_b200.so).
+/* dfvo_b200 -- C ABI of the H100-native DF-VO tracking hot path (libdfvo_b200.so).
  *
  * This is the drop-in boundary of SURVEY.md section 8(b): the reference is pure Python and has no
  * FFI of its own, so every entry point below names the reference *Python* interface it replaces
@@ -35,8 +35,8 @@ extern "C" {
 #define DFVO_NET_MONODEPTH2 1
 
 #define DFVO_PREC_FP32 0 /* every conv on CUDA cores in fp32 (parity mode)            */
-#define DFVO_PREC_BF16 1 /* bf16 activations, tcgen05 tensor-core convs, fp32 accum   */
-#define DFVO_PREC_TF32 2 /* fp32 activations, tcgen05 kind::tf32 convs, fp32 accum    */
+#define DFVO_PREC_BF16 1 /* bf16 activations, wgmma tensor-core convs, fp32 accum     */
+#define DFVO_PREC_TF32 2 /* fp32 activations, wgmma tf32 convs, fp32 accum            */
 
 #define DFVO_ACT_NONE 0
 #define DFVO_ACT_LEAKY 1 /* LeakyReLU(0.1) */
@@ -48,11 +48,11 @@ typedef struct dfvo_ctx dfvo_ctx;
 
 const char* dfvo_last_error(void);
 const char* dfvo_version(void);
-/* 1 if this library was built by nvcc for sm_100a, 0 for the CPU test build (tests/hostsim). */
+/* 1 if this library was built by nvcc for sm_90a, 0 for the CPU test build (tests/hostsim). */
 int dfvo_is_device_build(void);
 
 /* instrumentation for bench.py: number of kernel launches issued by this library so far (process-wide), and
- * CUDA-event timing of the tcgen05 conv launches while enabled (sum of durations in ms, launch count, and
+ * CUDA-event timing of the tensor-core conv launches while enabled (sum of durations in ms, launch count, and
  * algorithmic FLOPs = 2*MAC over real channels). */
 long long dfvo_launch_count(void);
 void dfvo_profile_enable(int on);
@@ -129,8 +129,8 @@ int dfvo_fb_consistency(const float* flow_fwd, const float* flow_bwd, float* dif
 int dfvo_fb_consistency_batch(const float* flow_fwd, const float* flow_bwd, float* diff, int n_pairs, int H, int W,
                               void* stream);
 /* torch.nn.Conv2d (+ activation): x [B,Cin,H,W], w_host [Cout,Cin,kh,kw], bias_host [Cout] or NULL
- * -> y [B,Cout,Ho,Wo].  precision DFVO_PREC_BF16 / DFVO_PREC_TF32 run the tcgen05 kernels (kind::f16 on bf16 operands /
- * kind::tf32 on fp32 operands; stride 1, or stride 2 on even sizes with 'same' padding). */
+ * -> y [B,Cout,Ho,Wo].  precision DFVO_PREC_BF16 / DFVO_PREC_TF32 run the wgmma kernels (bf16 operands /
+ * fp32 operands read as tf32; stride 1, or stride 2 on even sizes with 'same' padding). */
 int dfvo_conv2d(const float* x, const float* w_host, const float* bias_host, float* y, int B, int Cin,
                 int H, int W, int Cout, int kh, int kw, int stride, int pad_y, int pad_x, int reflect,
                 int act, int precision, void* stream);

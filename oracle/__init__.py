@@ -9,9 +9,8 @@ used exclusively as the *checker* for the CUDA path:
     CUDA library is missing instead of falling back to this code.
 
 Pinning status: the reference repository ships no tests, golden vectors or weights
-(SURVEY.md section 4), so the oracle is pinned against *outputs of the reference itself run
-in the build container* (``oracle/gen_golden.py`` imports ``/root/reference`` under
+(SURVEY.md section 4), so the oracle is pinned against *outputs of the reference itself*
+(``oracle/gen_golden.py`` imports a DF-VO checkout named by ``DFVO_REFERENCE_ROOT`` under
 ``oracle/shims.py`` and writes ``tests/golden/*.npz``), and against the third-party
-solvers the reference calls (``cv2`` 4.13.0, ``sklearn`` 1.9.0) which are present both
-here and on the GPU box.  See DESIGN.md "Oracle" for the per-function table.
+solvers the reference calls (``cv2`` 4.13.0, ``sklearn`` 1.9.0), which the tests import too.  See DESIGN.md "Oracle" for the per-function table.
 """

@@ -1,5 +1,5 @@
-"""Generate tests/golden/*.npz by running the REFERENCE ITSELF (imported from /root/reference under
-oracle/shims.py) on seeded synthetic inputs.  Build-container only.
+"""Generate tests/golden/*.npz by running the REFERENCE ITSELF (a DF-VO checkout named by DFVO_REFERENCE_ROOT, imported
+under oracle/shims.py) on seeded synthetic inputs.
 
     python -m oracle.gen_golden [name ...]
 

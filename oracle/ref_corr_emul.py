@@ -1,7 +1,7 @@
 """Run the REFERENCE's own correlation CUDA kernels on the CPU, from the source text where it
-lies (``/root/reference/libs/deep_models/flow/lite_flow_net/correlation.py:11-106``), to pin
-the oracle restatement ``oracle.nets.correlation``.  Build-container only (needs
-``/root/reference``); products go to ``oracle/_ref/`` (git-ignored).
+lies (``libs/deep_models/flow/lite_flow_net/correlation.py:11-106`` of the checkout), to pin
+the oracle restatement ``oracle.nets.correlation`` (needs
+a checkout named by ``DFVO_REFERENCE_ROOT``); products go to ``oracle/_ref/`` (git-ignored).
 
 How: the reference keeps its kernels as CUDA-C strings and specialises them per tensor shape
 with its own pure-Python ``cupy_kernel`` substitution (correlation.py:238-274).  We call that

@@ -1,7 +1,6 @@
-"""Import shims that let the UNMODIFIED reference (``/root/reference``) run on a CPU-only
-box with current library versions.  Used only by ``oracle/gen_golden.py`` (golden-vector
-generation, build container) -- never at test/bench time on the GPU box, where
-``/root/reference`` does not exist.
+"""Import shims that let the UNMODIFIED reference (a DF-VO checkout named by ``DFVO_REFERENCE_ROOT``) run on a
+CPU-only machine with current library versions.  Used only by ``oracle/gen_golden.py`` (golden-vector generation)
+and ``oracle/ref_corr_emul.py`` -- never at test or bench time.
 
 Each shim corresponds to one row of SURVEY.md Appendix B:
 
@@ -15,13 +14,14 @@ Each shim corresponds to one row of SURVEY.md Appendix B:
                                                                            -> oracle restatement
 """
 import importlib
+import os
 import sys
 import types
 
 import numpy as np
 import torch
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("DFVO_REFERENCE_ROOT", "")
 ALIGN_CORNERS_PINNED = True  # torch-1.1 semantics the reference was written for (SURVEY H3)
 
 _installed = False

@@ -1,4 +1,4 @@
-"""Drive single tcgen05 conv launches (LiteFlowNet level-2 shapes) for ncu."""
+"""Drive single tensor-core conv launches (LiteFlowNet level-2 shapes) for ncu."""
 import sys, os, ctypes
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "df-vo_b200")); sys.path.insert(0, os.path.join(ROOT, "tests"))

@@ -1,6 +1,6 @@
 """Small pass over every kernel family of the hot path, meant to run under compute-sanitizer (memcheck / racecheck / synccheck):
 LiteFlowNet (per-layer and chained convs, fused warp+correlation), monodepth2, consistency, selection, E / H / PnP RANSAC.
-No oracle here -- the parity tests do the checking; this run only has to be clean.  Usage (GPU box):
+No oracle here -- the parity tests do the checking; this run only has to be clean.  Usage (on a GPU):
   compute-sanitizer --tool memcheck python scripts/sanitize_run.py"""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""Per-layer CUDA-event times of every tcgen05 conv launch of one frame (development aid).
+"""Per-layer CUDA-event times of every tensor-core conv launch of one frame (development aid).
 Run with DFVO_TC_TRACE=1; the table goes to stderr."""
 import ctypes, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,14 +1,14 @@
 """Seeded synthetic inputs shared by golden generation, tests and bench (SURVEY.md 8d).
 
 Everything is produced from ``np.random.RandomState(seed)`` with a fixed draw order, so the
-build container and the GPU box regenerate bit-identical weights / frames / correspondences
+machine that generates goldens and every machine that tests regenerate bit-identical weights / frames / correspondences
 and only small *outputs* need to be committed under ``tests/golden/``.
 
 Weight dictionaries use the reference's own state-dict key names
 (``lite_flow_net.py:35-271`` -> ``moduleFeatures.moduleOne.0.weight`` ...;
 ``resnet_encoder.py:68-98`` / ``depth_decoder.py:30-47`` -> ``encoder.layer1.0.conv1.weight``,
 ``decoder.0.conv.conv.weight`` ...), so the same dict loads into the reference modules
-(golden generation) and into the B200 weight packer.
+(golden generation) and into the CUDA weight packer.
 """
 import math
 

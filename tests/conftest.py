@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "df-vo_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (runs on the B200 box only)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100)")
 
 
 @pytest.fixture(scope="session")

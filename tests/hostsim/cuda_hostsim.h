@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY -- never part of the product library.
 //
 // A tiny single-threaded emulation of the CUDA execution model, so that the *same* .cu sources
-// that nvcc compiles for sm_100a (every kernel except the tcgen05/TMA one) can also be compiled
+// that nvcc compiles for sm_90a (every kernel except the wgmma/TMA ones) can also be compiled
 // by g++ and exercised by the CPU test-suite in a container that has no GPU:
 //   * a kernel launch runs the blocks of the grid one after another;
 //   * the threads of a block are ucontext fibers; __syncthreads() yields to the scheduler, which

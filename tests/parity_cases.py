@@ -2,7 +2,7 @@
 device networks in every precision mode against the CPU oracle (torch fp32), and what the difference does downstream --
 bits of the `flow_diff < 0.1` mask, members of the local_bestN keypoint set, the recovered pose.
 
-Used by tests/test_gpu_parity_fullsize.py (asserts the bounds, writes the table to gpurun_out/parity_fullsize.json) and by
+Used by tests/test_gpu_parity_fullsize.py (asserts the bounds, writes the table to $DFVO_REPORT_DIR/parity_fullsize.json) and by
 `bench.py --config parity` (prints the same table).  The oracle is the checker only.
 
 End-to-end chain.  There are no trained weights offline, and a random-weight LiteFlowNet has no forward-backward-consistent
@@ -238,8 +238,11 @@ def measure_all(lib, engine, modes=None, seeds=CHAIN_SEEDS):
 
 
 def write_report(table, name="parity_fullsize.json"):
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    d = os.path.join(root, "gpurun_out")
+    """Writes the table as JSON into the directory DFVO_REPORT_DIR names; nothing is written when it is unset (the test prints
+    the table either way), so a test run leaves the source tree as it found it."""
+    d = os.environ.get("DFVO_REPORT_DIR")
+    if not d:
+        return
     os.makedirs(d, exist_ok=True)
     with open(os.path.join(d, name), "w") as f:
         json.dump(table, f, indent=1, sort_keys=True)

@@ -36,7 +36,7 @@ def test_product_library_exports_all_and_is_device_build():
     for s in header_symbols():
         assert hasattr(lib.cdll, s)
     assert lib.dfvo_is_device_build() == 1
-    assert b"sm_100a" in lib.dfvo_version()
+    assert b"sm_90a" in lib.dfvo_version()
 
 
 def test_product_loader_refuses_without_cuda():

@@ -1,5 +1,5 @@
-"""CPU: tests/vo_driver.py -- the reference driver's call sequence restated for the GPU box, where libs/dfvo.py does not
-exist -- reproduces the goldens the UNMODIFIED driver produced (tests/golden/dfvo_driver_*.npz), so the GPU drop-in test
+"""CPU: tests/vo_driver.py -- the reference driver's call sequence restated for machines without a DF-VO checkout (libs/dfvo.py
+is not part of this repository) -- reproduces the goldens the UNMODIFIED driver produced (tests/golden/dfvo_driver_*.npz), so the GPU drop-in test
 (test_gpu_dropin.py) is anchored on the reference's own output.  Kernels run in the host-emulation build; the two networks
 are replaced by the analytic frame inputs here (their emulation takes minutes) and run for real in the GPU test."""
 import os

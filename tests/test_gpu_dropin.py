@@ -1,4 +1,4 @@
-"""GPU: the drop-in boundary on real hardware (SURVEY 8b), without /root/reference: tests/vo_driver.py replays the call
+"""GPU: the drop-in boundary on real hardware (SURVEY 8b), without a DF-VO checkout: tests/vo_driver.py replays the call
 sequence of libs/dfvo.py against the UN-PATCHED mirror -- DeepModel.initialize_models (torch.load of checkpoints written
 with torch.save) -> forward_depth / forward_flow (device-backed arrays) -> KeypointSampler -> EssTracker / PnpTracker.
 

@@ -66,7 +66,7 @@ def test_liteflow_full_size_properties(dev_lib):
 
 def test_liteflow_two_pairs_batched(dev_lib):
     """Batched many-pairs mode (BASELINE configs[2] / SURVEY 8e): two independent pairs in one forward == each pair alone,
-    bit for bit (tcgen05 path, bf16)."""
+    bit for bit (wgmma path, bf16)."""
     H, W = 128, 416
     imgs = [synth.value_noise_image(H, W, s) for s in (1, 2, 3, 4)]
     w = synth.liteflownet_weights()

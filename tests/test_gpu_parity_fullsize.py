@@ -1,7 +1,7 @@
 """GPU: precision-mode parity at the BASELINE sizes (VERDICT r1 "What's weak" 1): the product networks in every precision
-mode (fp32 CUDA-core, tf32 tcgen05, bf16 tcgen05) against the CPU oracle at 376x1241 (flow) and 192x640 (depth), and the
+mode (fp32 CUDA-core, tf32 wgmma, bf16 wgmma) against the CPU oracle at 376x1241 (flow) and 192x640 (depth), and the
 downstream effect of the difference on mask bits, selected keypoints and the pose (tests/parity_cases.py explains the
-end-to-end construction).  The table is written to gpurun_out/parity_fullsize.json; DESIGN.md section 5 quotes it.
+end-to-end construction).  The table is printed, and written to $DFVO_REPORT_DIR/parity_fullsize.json when that is set.
 
 Tolerances (floating point; the tolerance is the assertion):
   fp32 mode : flow EPE max < 1e-3 px, |d flow_diff| max < 2e-3 px, depth rel < 1e-4           (summation order only)

@@ -2,7 +2,7 @@
 
 Tolerances (floating point, SURVEY 8a / H4):
   * fp32 kernels vs fp32 oracle: 2e-5 abs on O(1) data (summation order only);
-  * bf16/tcgen05 kernels vs an fp32 oracle evaluated on bf16-rounded operands: 1e-2 relative
+  * bf16/wgmma kernels vs an fp32 oracle evaluated on bf16-rounded operands: 1e-2 relative
     (fp32 accumulation, outputs rounded to bf16).
 """
 import ctypes
@@ -190,7 +190,7 @@ TC_CASES = [
 
 # the level-2 layers that carry 69 % of the frame's FLOPs (176x608x2, multi-wave persistent CTAs, S = 2 / 4 sub-tiles)
 TC_BIG_CASES = [
-    (2, 128, 176, 608, 128, 3, 3, 1, 1, 1),    # S = 2, block_n 128, 836 tiles over 148 CTAs
+    (2, 128, 176, 608, 128, 3, 3, 1, 1, 1),    # S = 2, block_n 128, 836 tiles over the persistent CTAs
     (2, 130, 176, 608, 128, 3, 3, 1, 1, 1),    # Subpixel Main.0: 144-channel input with a partial last chunk
     (2, 128, 176, 608, 64, 3, 3, 1, 1, 1),     # S = 4, block_n 64
     (2, 64, 176, 608, 32, 3, 3, 1, 1, 1),      # S = 4, block_n 32
@@ -232,7 +232,7 @@ def tf32_round(x):
 
 
 def _tc_conv_check(dev_lib, case, prec, stride=1):
-    """tcgen05 conv (prec 1: kind::f16 on bf16 operands; prec 2: kind::tf32 on fp32 operands) vs an fp64 convolution of the
+    """wgmma conv (prec 1: bf16 operands; prec 2: fp32 operands read as tf32) vs an fp64 convolution of the
     operands rounded to the tensor core's input format.  Tolerances: bf16 output rounding 2^-9; tf32 mode stores fp32
     rounded to tf32 (2^-11) and the activations are rounded once more on the way in."""
     B, Cin, H, W, Cout, kh, kw, py, px, act = case

@@ -1,7 +1,7 @@
 """CPU: the library's own .cu sources compiled for the host against an emulation of the CUDA execution
 model (tests/hostsim) -- validates kernel indexing, layouts, weight packing and the network / RANSAC
 orchestration against the oracle and the reference-generated goldens before GPU time is spent.
-(The tcgen05 kernel itself cannot run here; its host emulation consumes the same ConvTc description and
+(The wgmma kernels themselves cannot run here; its host emulation consumes the same ConvTc description and
 packed weights, so the bf16 plumbing is covered, the PTX is covered by tests/test_gpu_*.py.)"""
 import ctypes
 import os
@@ -103,7 +103,7 @@ def test_liteflownet_bf16_plumbing(hostsim_lib):
 
 def test_tf32_mode_plumbing(hostsim_lib):
     """DFVO_PREC_TF32 wiring (fp32 activations, layers packed for 4-byte tensor-core operands, im2row stem, CUDA-core heads):
-    in the CPU emulation the tcgen05 kind::tf32 convs are exact fp32 arithmetic on tf32-rounded weights, so both networks must
+    in the CPU emulation the wgmma tf32 convs are exact fp32 arithmetic on tf32-rounded weights, so both networks must
     land within tf32 weight-rounding distance of the reference goldens."""
     g = np.load(os.path.join(G, "deep_models_70x150.npz"))
     H, W = 70, 150

@@ -1,6 +1,5 @@
 """CPU: the oracle restatements (oracle/nets.py, oracle/vo.py) against golden vectors produced by
-the reference itself (oracle/gen_golden.py, run in the build container where /root/reference is
-mounted).  This is what pins the oracle (SURVEY 8c: the reference ships no tests of its own)."""
+the reference itself (oracle/gen_golden.py, run against a DF-VO checkout named by DFVO_REFERENCE_ROOT).  This is what pins the oracle (SURVEY 8c: the reference ships no tests of its own)."""
 import os
 
 import numpy as np

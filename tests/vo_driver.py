@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE: the per-frame call sequence of the reference driver (libs/dfvo.py), hybrid tracking, restated as a
-small loop so that the drop-in tests can run on the GPU box, where /root/reference (and therefore libs/dfvo.py itself)
+small loop so that the drop-in tests can run without a DF-VO checkout (and therefore without libs/dfvo.py itself)
 does not exist.  It touches the `libs.*` mirror only through the calls the real driver makes, in the same order:
 
     DFVO.setup            dfvo.py:60-92    Dataset -> trackers -> KeypointSampler -> DeepModel(cfg).initialize_models()
