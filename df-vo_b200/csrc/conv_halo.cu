@@ -186,11 +186,16 @@ static bool halo_fit(int S, int bn, int kh, int kw, int Cout_pad, HaloCfg* out) 
   return true;
 }
 
-// Pick (S, block_n): minimise  waves x max(MMA time, L2->SM time)  per tile + a fixed per-tile overhead.  An estimate from the
-// H100 SXM data sheet, not a measurement: per K=16 step of the 128-pixel sub-tile, MMA time = max(block_n, 32 + block_n / 2) clk
-// (tensor rate of ~2048 bf16 MACs / clk / SM vs shared-memory operand reads at 128 B / clk); L2 -> SM ~25 B/clk per SM when every
-// SM streams (~3.3 KB / clk for the chip), up to ~5x that for a lone CTA.  block_n is one of the wgmma shapes 16 .. 256 and
-// S * block_n <= 256 keeps the accumulators of a consumer thread at <= 128 registers.
+// Pick (S, block_n): minimise  waves x (max(MMA time, L2->SM time) + epilogue + per-tile bubble)  per tile.  The MMA term is the
+// data-sheet rate: per K=16 step of the 128-pixel sub-tile max(block_n, 32 + block_n / 2) clk (~2048 bf16 MACs / clk / SM vs
+// shared-memory operand reads at 128 B / clk).  The other constants are fitted to measurements, not data-sheet figures: every
+// (S, block_n) of the LiteFlowNet level-2 / level-3 layer shapes of scripts/conv_shapes.py timed with CUDA events on one H100
+// 80GB HBM3 at a 400 W power limit (DFVO_HALO_S / DFVO_HALO_BN force a configuration).  The epilogue, which runs after the
+// tile's last MMA and stores from the accumulator fragment, costs S * block_n * (150 + 0.6 * S * block_n) clk per tile: it, not
+// the L2 -> SM traffic, is most of a large tile's time.  S * block_n = 64 (S = 1 / block_n = 64, S = 2 / block_n = 32) was the
+// fastest configuration on every measured shape and no larger tile was faster on any, so the candidates stop at
+// S * block_n = 64 (a consumer thread holds <= 32 accumulators).  L2 -> SM ~5 KB / clk for the chip shared by the active CTAs
+// (at most 128 B / clk for one); ~3000 clk per-tile bubble.  block_n is one of the wgmma shapes 16, 32, 64.
 static bool halo_choose(const ConvTc& c, int kh, int kw, HaloCfg* best) {
   int ktot16 = 0, kbytes = 0;                       // 32-byte K steps and bytes per pixel over all sources
   const int es = c.esize == 4 ? 4 : 2;
@@ -200,8 +205,8 @@ static bool halo_choose(const ConvTc& c, int kh, int kw, HaloCfg* best) {
   bool found = false;
   for (int S = 1; S <= 4; S <<= 1) {
     if (fS && S != fS) continue;
-    for (int bn = 16; bn <= 256 && bn <= c.Cout_pad; bn <<= 1) {
-      if (c.Cout_pad % bn || S * bn > 256) continue;
+    for (int bn = 16; S * bn <= 64 && bn <= c.Cout_pad; bn <<= 1) {
+      if (c.Cout_pad % bn) continue;
       if (fN && bn != fN) continue;
       HaloCfg h;
       if (!halo_fit(S, bn, kh, kw, c.Cout_pad, &h)) continue;
@@ -210,11 +215,11 @@ static bool halo_choose(const ConvTc& c, int kh, int kw, HaloCfg* best) {
       const int active = (int)(tiles < nsm ? tiles : nsm);
       const double mma = (double)ktot16 * kh * kw * S * ((bn > 32 + bn / 2.0) ? bn : 32 + bn / 2.0);
       const double bytes = (double)(8 * S + kw - 1) * (HALO_TH + kh - 1) * kbytes + (double)kh * kw * bn * kbytes;
-      double bw = 3300.0 / active; if (bw > 128.0) bw = 128.0;
+      double bw = 5000.0 / active; if (bw > 128.0) bw = 128.0;
       const double l2 = bytes / bw;
-      const double epi = (double)S * bn * 10.0;                 // ~epilogue clk per tile (not overlapped with the MMAs)
+      const double epi = (double)S * bn * (150.0 + 0.6 * S * bn);   // epilogue clk per tile (not overlapped with the MMAs)
       const double tile = (mma > l2 ? mma : l2) + epi;
-      h.cost = (double)waves * (tile + 1500.0) + 4000.0;        // per-tile pipeline bubble, per-launch prologue
+      h.cost = (double)waves * (tile + 3000.0) + 4000.0;        // per-tile pipeline bubble, per-launch prologue
       if (!found || h.cost < best->cost) { *best = h; found = true; }
     }
   }
@@ -247,9 +252,7 @@ template <int TF32>
 static int launch_halo_t(int S, int bn, const CUtensorMap* tmA, const CUtensorMap& tmB, const ConvHaloK& k, int grid, size_t smem,
                          cudaStream_t s) {
 #define DFVO_HALO_CASE(SS, NN) if (S == SS && bn == NN) return launch_halo<SS, NN, TF32>(tmA, tmB, k, grid, smem, s);
-  DFVO_HALO_CASE(1, 16) DFVO_HALO_CASE(1, 32) DFVO_HALO_CASE(1, 64) DFVO_HALO_CASE(1, 128) DFVO_HALO_CASE(1, 256)
-  DFVO_HALO_CASE(2, 16) DFVO_HALO_CASE(2, 32) DFVO_HALO_CASE(2, 64) DFVO_HALO_CASE(2, 128)
-  DFVO_HALO_CASE(4, 16) DFVO_HALO_CASE(4, 32) DFVO_HALO_CASE(4, 64)
+  DFVO_HALO_CASE(1, 16) DFVO_HALO_CASE(1, 32) DFVO_HALO_CASE(1, 64) DFVO_HALO_CASE(2, 16) DFVO_HALO_CASE(2, 32) DFVO_HALO_CASE(4, 16)
 #undef DFVO_HALO_CASE
   DFVO_REQUIRE(false, DFVO_EINVAL, "conv_halo: no kernel for S %d block_n %d", S, bn);
 }
