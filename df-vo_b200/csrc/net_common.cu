@@ -217,7 +217,7 @@ int run_conv_multi(const ConvLayer& L, const Ten<const T>* ins, int nin, Ten<T> 
   c.N = ins[0].N; c.H = out.H; c.W = out.W; c.inH = ins[0].H; c.inW = ins[0].W; c.stride = 1; c.nsrc = nin;
   fill_taps(L, &c);
   c.esize = L.tc_esize; c.round_out_tf32 = sizeof(T) == 4;
-  c.w = L.w_tc; c.Cout_pad = L.Cout_pad; c.Cout = L.Cout; c.bias = L.bias; c.act = act; c.out_f32 = 0;
+  c.w = L.w_tc; c.Cout_pad = L.Cout_pad; c.Cout = L.Cout; c.bias = L.bias; c.act = act; c.out_f32 = sizeof(T) == 4;
   c.out = out.p; c.oN = out.sN; c.oH = out.sH; c.oW = out.sW;
   c.flops = flops > 0 ? flops : 2.0 * (double)c.N * out.H * out.W * (double)L.Cout * L.Cin_ref * L.kh * L.kw;
   return conv_tc(c, s);
