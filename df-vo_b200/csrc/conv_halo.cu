@@ -13,7 +13,8 @@
 //     weights cross L2 -> SM once per 128*S pixels;
 //   * A and B have their own mbarrier rings and producer warps (a B slot is freed per tap, an A slot per chunk).
 // Warp roles: 0 = A producer (TMA), 1 = B producer (TMA), 2-3 idle; warpgroups 1 and 2 = consumers (wgmma for pixel rows 0-7 / 8-15
-// of every sub-tile, accumulators in registers, then the epilogue).  tc_ptx.cuh::halo_tile_mma is the MMA loop.
+// of every sub-tile, accumulators in registers, then the epilogue).  tc_ptx.cuh::halo_tile_mma is the MMA loop.  One or two CTAs
+// run per SM (MINB): with two, one CTA's epilogue runs while the other's MMAs keep the tensor pipe busy.
 // Restates torch.nn.Conv2d(stride=1) + LeakyReLU/ELU/ReLU as used at lite_flow_net.py:98-240 and
 // depth_decoder.py / torchvision BasicBlock (BN folded by the weight packer), like conv_tc.cu.
 #include "tc_ptx.cuh"
@@ -43,8 +44,8 @@ struct ConvHaloK {
 #define HALO_THREADS 384
 #define HALO_TH 16
 
-template <int S, int BN, int TF32>
-__global__ void __launch_bounds__(HALO_THREADS, 1)
+template <int S, int BN, int TF32, int MINB>
+__global__ void __launch_bounds__(HALO_THREADS, MINB)
 k_conv_halo(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
             const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ ConvHaloK p) {
@@ -164,16 +165,17 @@ static bool rect_taps(const ConvTc& c, int* kh, int* kw, int* dy0, int* dx0) {
   return true;
 }
 
-struct HaloCfg { int S, block_n, a_stages, b_stages, a_stage_bytes; size_t smem; double cost; };
+struct HaloCfg { int S, block_n, ctas, a_stages, b_stages, a_stage_bytes; size_t smem; double cost; };
 
-// shared memory: A ring + B ring + barriers + bias (+ 1 KB alignment slack)
-static bool halo_fit(int S, int bn, int kh, int kw, int Cout_pad, HaloCfg* out) {
+// shared memory: A ring + B ring + barriers + bias (+ 1 KB alignment slack), within 220 KB for one CTA per SM or 110 KB each
+// for two
+static bool halo_fit(int S, int bn, int ctas, int kh, int kw, int Cout_pad, HaloCfg* out) {
   const int HW = 8 * S + kw - 1, HH = HALO_TH + kh - 1;
   if (HW > 256 || HH > 256) return false;
   const int a_stage = (HW * HH * 128 + 1023) & ~1023;
   const int b_stage = bn * 128;
   const size_t fixed = 1024 + 8 * 64 + (size_t)Cout_pad * 4;      // alignment slack, <= 30 barriers, bias
-  const size_t budget = 220 * 1024;
+  const size_t budget = (size_t)(220 / ctas) * 1024;
   int a_stages = 2, b_stages = 2;
   if (fixed + (size_t)a_stages * a_stage + (size_t)b_stages * b_stage > budget) return false;
   // a B slot lives for one tap (S MMAs per K step), an A slot for a whole chunk (kh*kw taps): two A slots already cover the
@@ -181,46 +183,57 @@ static bool halo_fit(int S, int bn, int kh, int kw, int Cout_pad, HaloCfg* out) 
   while (b_stages < 8 && fixed + (size_t)a_stages * a_stage + (size_t)(b_stages + 1) * b_stage <= budget) ++b_stages;
   while (a_stages < 3 && fixed + (size_t)(a_stages + 1) * a_stage + (size_t)b_stages * b_stage <= budget) ++a_stages;
   while (b_stages < 12 && fixed + (size_t)a_stages * a_stage + (size_t)(b_stages + 1) * b_stage <= budget) ++b_stages;
-  out->S = S; out->block_n = bn; out->a_stages = a_stages; out->b_stages = b_stages; out->a_stage_bytes = a_stage;
+  out->S = S; out->block_n = bn; out->ctas = ctas; out->a_stages = a_stages; out->b_stages = b_stages; out->a_stage_bytes = a_stage;
   out->smem = fixed + (size_t)a_stages * a_stage + (size_t)b_stages * b_stage;
   return true;
 }
 
-// Pick (S, block_n): minimise  waves x (max(MMA time, L2->SM time) + epilogue + per-tile bubble)  per tile.  The MMA term is the
-// data-sheet rate: per K=16 step of the 128-pixel sub-tile max(block_n, 32 + block_n / 2) clk (~2048 bf16 MACs / clk / SM vs
-// shared-memory operand reads at 128 B / clk).  The other constants are fitted to measurements, not data-sheet figures: every
-// (S, block_n) of the LiteFlowNet level-2 / level-3 layer shapes of scripts/conv_shapes.py timed with CUDA events on one H100
-// 80GB HBM3 at a 400 W power limit (DFVO_HALO_S / DFVO_HALO_BN force a configuration).  The epilogue, which runs after the
-// tile's last MMA and stores from the accumulator fragment, costs S * block_n * (150 + 0.6 * S * block_n) clk per tile: it, not
-// the L2 -> SM traffic, is most of a large tile's time.  S * block_n = 64 (S = 1 / block_n = 64, S = 2 / block_n = 32) was the
-// fastest configuration on every measured shape and no larger tile was faster on any, so the candidates stop at
-// S * block_n = 64 (a consumer thread holds <= 32 accumulators).  L2 -> SM ~5 KB / clk for the chip shared by the active CTAs
-// (at most 128 B / clk for one); ~3000 clk per-tile bubble.  block_n is one of the wgmma shapes 16, 32, 64.
+// Pick (S, block_n, CTAs per SM): minimise  waves x (time of one wave)  + launch prologue.  One tile's tensor-pipe time is
+//   busy = max(MMA, L2 -> SM) + 200 clk per (channel chunk, tap) wgmma group,
+// and after its last MMA the tile's epilogue (200 clk per unit of S * block_n) and a ~1000 clk pipeline bubble follow.  One CTA
+// per SM runs busy + epilogue + bubble per wave; two CTAs per SM run a pair of tiles per wave in max(2 busy, 1.3 x (busy +
+// epilogue + bubble)): the warp schedulers run one CTA's epilogue while the other's MMAs keep the tensor pipe busy, at the
+// price of each tile running slower than alone.  The MMA term is the data-sheet rate: per K=16 step of the 128-pixel sub-tile
+// max(block_n, 32 + block_n / 2) clk (~2048 bf16 MACs / clk / SM vs shared-memory operand reads at 128 B / clk).  The other
+// constants are fitted, not data-sheet figures: every (S, block_n, CTAs) of the LiteFlowNet level-2 / level-3 layer shapes of
+// scripts/conv_shapes.py timed with CUDA events on one H100 80GB HBM3 at a 400 W power limit (DFVO_HALO_S / DFVO_HALO_BN /
+// DFVO_HALO_CTAS force a configuration).  The fit puts the chip's L2 -> SM rate at >= 20 KB / clk (at most 128 B / clk per
+// SM): the operand traffic does not bound these tiles.  S * block_n = 128 (block_n 128 at S = 1, 64 at S = 2, 32 at S = 4)
+// was slower than S * block_n = 64 on every measured shape, so the candidates stop at S * block_n = 64 (a consumer thread
+// holds <= 32 accumulators, which also keeps two CTAs within 80 registers per thread).  block_n is one of the wgmma shapes
+// 16, 32, 64.
 static bool halo_choose(const ConvTc& c, int kh, int kw, HaloCfg* best) {
-  int ktot16 = 0, kbytes = 0;                       // 32-byte K steps and bytes per pixel over all sources
+  int ktot16 = 0, kbytes = 0, chunks = 0;           // 32-byte K steps, bytes per pixel and 128-byte channel chunks over all sources
   const int es = c.esize == 4 ? 4 : 2;
-  for (int s = 0; s < c.nsrc; ++s) { ktot16 += (c.src[s].C * es + 31) / 32; kbytes += c.src[s].C * es; }
+  for (int s = 0; s < c.nsrc; ++s) {
+    ktot16 += (c.src[s].C * es + 31) / 32; kbytes += c.src[s].C * es; chunks += (c.src[s].C * es + 127) / 128;
+  }
   const int nsm = tc_num_sms();
-  const int fS = env_int("DFVO_HALO_S", 0), fN = env_int("DFVO_HALO_BN", 0);
+  const int fS = env_int("DFVO_HALO_S", 0), fN = env_int("DFVO_HALO_BN", 0), fC = env_int("DFVO_HALO_CTAS", 0);
   bool found = false;
-  for (int S = 1; S <= 4; S <<= 1) {
-    if (fS && S != fS) continue;
-    for (int bn = 16; S * bn <= 64 && bn <= c.Cout_pad; bn <<= 1) {
-      if (c.Cout_pad % bn) continue;
-      if (fN && bn != fN) continue;
-      HaloCfg h;
-      if (!halo_fit(S, bn, kh, kw, c.Cout_pad, &h)) continue;
-      const long long tiles = (long long)cdiv(c.W, 8 * S) * cdiv(c.H, HALO_TH) * c.N * (c.Cout_pad / bn);
-      const long long waves = (tiles + nsm - 1) / nsm;
-      const int active = (int)(tiles < nsm ? tiles : nsm);
-      const double mma = (double)ktot16 * kh * kw * S * ((bn > 32 + bn / 2.0) ? bn : 32 + bn / 2.0);
-      const double bytes = (double)(8 * S + kw - 1) * (HALO_TH + kh - 1) * kbytes + (double)kh * kw * bn * kbytes;
-      double bw = 5000.0 / active; if (bw > 128.0) bw = 128.0;
-      const double l2 = bytes / bw;
-      const double epi = (double)S * bn * (150.0 + 0.6 * S * bn);   // epilogue clk per tile (not overlapped with the MMAs)
-      const double tile = (mma > l2 ? mma : l2) + epi;
-      h.cost = (double)waves * (tile + 3000.0) + 4000.0;        // per-tile pipeline bubble, per-launch prologue
-      if (!found || h.cost < best->cost) { *best = h; found = true; }
+  for (int ctas = 1; ctas <= 2; ++ctas) {
+    if (fC && ctas != fC) continue;
+    for (int S = 1; S <= 4; S <<= 1) {
+      if ((fS && S != fS) || (ctas == 2 && S == 4)) continue;   // two A slots of an S = 4 halo do not fit in 110 KB
+      for (int bn = 16; S * bn <= 64 && bn <= c.Cout_pad; bn <<= 1) {
+        if (c.Cout_pad % bn) continue;
+        if (fN && bn != fN) continue;
+        HaloCfg h;
+        if (!halo_fit(S, bn, ctas, kh, kw, c.Cout_pad, &h)) continue;
+        const long long tiles = (long long)cdiv(c.W, 8 * S) * cdiv(c.H, HALO_TH) * c.N * (c.Cout_pad / bn);
+        const long long slots = (long long)ctas * nsm;
+        const long long waves = (tiles + slots - 1) / slots;
+        const int active = (int)(tiles < slots ? tiles : slots);
+        const double mma = (double)ktot16 * kh * kw * S * ((bn > 32 + bn / 2.0) ? bn : 32 + bn / 2.0);
+        const double bytes = (double)(8 * S + kw - 1) * (HALO_TH + kh - 1) * kbytes + (double)kh * kw * bn * kbytes;
+        double bw = 20000.0 / active; if (bw > 128.0 / ctas) bw = 128.0 / ctas;
+        const double l2 = bytes / bw;
+        const double busy = (mma > l2 ? mma : l2) + 200.0 * chunks * kh * kw;
+        const double serial = busy + 200.0 * S * bn + 1000.0;       // + epilogue + per-tile bubble
+        const double wave = ctas == 1 ? serial : (2.0 * busy > 1.3 * serial ? 2.0 * busy : 1.3 * serial);
+        h.cost = (double)waves * wave + 4000.0;                     // + per-launch prologue
+        if (!found || h.cost < best->cost) { *best = h; found = true; }
+      }
     }
   }
   return found;
@@ -235,26 +248,30 @@ bool conv_halo_supported(const ConvTc& c) {
   return halo_choose(c, kh, kw, &h);
 }
 
-template <int S, int BN, int TF32>
+template <int S, int BN, int TF32, int MINB>
 static int launch_halo(const CUtensorMap* tmA, const CUtensorMap& tmB, const ConvHaloK& k, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<S, BN, TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<S, BN, TF32, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    // two CTAs per SM need the largest shared-memory carve-out of the unified L1 / shared storage
+    if (MINB == 2)
+      DFVO_CUDA(cudaFuncSetAttribute(k_conv_halo<S, BN, TF32, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     attr_set = true;
   }
   cudaLaunchConfig_t cfg; cudaLaunchAttribute attr;
   tc_launch_config(&cfg, &attr, grid, HALO_THREADS, smem, s);
-  DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<S, BN, TF32>, tmA[0], tmA[1], tmA[2], tmB, k));
+  DFVO_CUDA(cudaLaunchKernelEx(&cfg, k_conv_halo<S, BN, TF32, MINB>, tmA[0], tmA[1], tmA[2], tmB, k));
   return DFVO_OK;
 }
 
 template <int TF32>
-static int launch_halo_t(int S, int bn, const CUtensorMap* tmA, const CUtensorMap& tmB, const ConvHaloK& k, int grid, size_t smem,
+static int launch_halo_t(int S, int bn, int ctas, const CUtensorMap* tmA, const CUtensorMap& tmB, const ConvHaloK& k, int grid, size_t smem,
                          cudaStream_t s) {
-#define DFVO_HALO_CASE(SS, NN) if (S == SS && bn == NN) return launch_halo<SS, NN, TF32>(tmA, tmB, k, grid, smem, s);
-  DFVO_HALO_CASE(1, 16) DFVO_HALO_CASE(1, 32) DFVO_HALO_CASE(1, 64) DFVO_HALO_CASE(2, 16) DFVO_HALO_CASE(2, 32) DFVO_HALO_CASE(4, 16)
+#define DFVO_HALO_CASE(SS, NN, CC) if (S == SS && bn == NN && ctas == CC) return launch_halo<SS, NN, TF32, CC>(tmA, tmB, k, grid, smem, s);
+  DFVO_HALO_CASE(1, 16, 1) DFVO_HALO_CASE(1, 32, 1) DFVO_HALO_CASE(1, 64, 1) DFVO_HALO_CASE(2, 16, 1) DFVO_HALO_CASE(2, 32, 1) DFVO_HALO_CASE(4, 16, 1)
+  DFVO_HALO_CASE(1, 16, 2) DFVO_HALO_CASE(1, 32, 2) DFVO_HALO_CASE(1, 64, 2) DFVO_HALO_CASE(2, 16, 2) DFVO_HALO_CASE(2, 32, 2)
 #undef DFVO_HALO_CASE
-  DFVO_REQUIRE(false, DFVO_EINVAL, "conv_halo: no kernel for S %d block_n %d", S, bn);
+  DFVO_REQUIRE(false, DFVO_EINVAL, "conv_halo: no kernel for S %d block_n %d with %d CTAs per SM", S, bn, ctas);
 }
 
 int conv_halo(const ConvTc& c, cudaStream_t s) {
@@ -304,17 +321,18 @@ int conv_halo(const ConvTc& c, cudaStream_t s) {
     int rc = tc_encode_map(&tmB, c.w, 3, dims, str, box, es);
     if (rc) return rc;
   }
-  const int grid = k.ntiles < tc_num_sms() ? k.ntiles : tc_num_sms();
+  const int slots = h.ctas * tc_num_sms();                       // persistent grid: ctas CTAs per SM
+  const int grid = k.ntiles < slots ? k.ntiles : slots;
   ++g_launch_count;
   TcProf pr;
   const bool prof = tc_prof_begin(s, &pr);
-  const int rc = es == 4 ? launch_halo_t<1>(S, bn, tmA, tmB, k, grid, h.smem, s) : launch_halo_t<0>(S, bn, tmA, tmB, k, grid, h.smem, s);
+  const int rc = es == 4 ? launch_halo_t<1>(S, bn, h.ctas, tmA, tmB, k, grid, h.smem, s) : launch_halo_t<0>(S, bn, h.ctas, tmA, tmB, k, grid, h.smem, s);
   if (rc) return rc;
   if (prof) {
     char d[256];
-    snprintf(d, sizeof(d), "halo%s N%d %dx%d k%dx%d src[%d,%d,%d] cout%d/%d bn%d S%d stages%d/%d grid%d tiles%d gflop %.3f", es == 4 ? "-tf32" : "", c.N, c.H, c.W,
+    snprintf(d, sizeof(d), "halo%s N%d %dx%d k%dx%d src[%d,%d,%d] cout%d/%d bn%d S%d stages%d/%d grid%d tiles%d ctas%d gflop %.3f", es == 4 ? "-tf32" : "", c.N, c.H, c.W,
              k.kh, k.kw, c.src[0].C, c.nsrc > 1 ? c.src[1].C : 0, c.nsrc > 2 ? c.src[2].C : 0, c.Cout, c.Cout_pad, bn,
-             S, k.a_stages, k.b_stages, grid, k.ntiles, c.flops * 1e-9);
+             S, k.a_stages, k.b_stages, grid, k.ntiles, h.ctas, c.flops * 1e-9);
     tc_prof_end(s, pr, c.flops, d);
   }
   DFVO_CHECK_LAUNCH();

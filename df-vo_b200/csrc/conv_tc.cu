@@ -62,6 +62,16 @@ struct ConvTcK {
 #define TC_THREADS 384
 #define TC_A_BYTES 16384
 
+// the MMAs of one ring stage as one wgmma group, then wait until at most this group is in flight
+template <int BN, int TF32, int NKS>
+__device__ __forceinline__ void tc_stage_mma(float (&acc)[1][BN / 2], uint32_t at, uint32_t bt, uint32_t fresh) {
+  using namespace tc;
+  wgmma_fence();
+  halo_tap_mma<1, BN, TF32, NKS>(acc, at, bt, 1024u, fresh);
+  wgmma_commit();
+  wgmma_wait<1>();
+}
+
 template <int BN, int TF32>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
@@ -140,20 +150,18 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
         for (int s = 0; s < p.nsrc; ++s) {
           for (int c0 = 0; c0 < p.srcC[s]; c0 += p.chunk) {
             mbar_wait(full_bar(stage), phase);
-            wgmma_fence();
             const uint32_t sa = base + (uint32_t)stage * stage_bytes;
             const int rem = p.srcC[s] - c0;
             const int nks = ((rem >= p.chunk ? p.chunk : rem) * p.esize) >> 5;       // 32-byte K steps with real channels
             float (&acc1)[1][BN / 2] = reinterpret_cast<float (&)[1][BN / 2]>(acc);
             const uint32_t at = sa + (uint32_t)wg * 8192u, bt = sa + TC_A_BYTES;   // the same K-step walk as one halo tap, S = 1
+            // one whole fence ... wait group per case (see tc_ptx.cuh::halo_chunk_mma): no run-time branch inside a wgmma group
             switch (nks) {
-              case 4: halo_tap_mma<1, BN, TF32, 4>(acc1, at, bt, 1024u, fresh); break;
-              case 3: halo_tap_mma<1, BN, TF32, 3>(acc1, at, bt, 1024u, fresh); break;
-              case 2: halo_tap_mma<1, BN, TF32, 2>(acc1, at, bt, 1024u, fresh); break;
-              default: halo_tap_mma<1, BN, TF32, 1>(acc1, at, bt, 1024u, fresh); break;
-            }
-            wgmma_commit();
-            wgmma_wait<1>();                                                          // the previous stage's MMAs are done
+              case 4: tc_stage_mma<BN, TF32, 4>(acc1, at, bt, fresh); break;
+              case 3: tc_stage_mma<BN, TF32, 3>(acc1, at, bt, fresh); break;
+              case 2: tc_stage_mma<BN, TF32, 2>(acc1, at, bt, fresh); break;
+              default: tc_stage_mma<BN, TF32, 1>(acc1, at, bt, fresh); break;
+            }                                                                         // the previous stage's MMAs are done: release it
             if (pend >= 0 && leader) mbar_arrive(empty_bar(pend));
             pend = stage;
             fresh = 1u;

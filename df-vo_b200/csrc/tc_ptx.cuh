@@ -158,6 +158,32 @@ __device__ __forceinline__ void halo_tap_mma(float (&acc)[S][BN / 2], uint32_t a
                            ks == 0 ? fresh : 1u);
 }
 
+// The taps of one (source, channel chunk) of a halo tile, NKS K steps each.  NKS is a template parameter and every tap's
+// fence -> MMAs -> commit -> wait<1> is one basic block: a run-time branch between the fence and the commit makes ptxas close a
+// wgmma group inside each branch and insert an empty one at the commit (C7519 "warpgroup.arrive is injected"), so wait<1>
+// would keep only that empty group in flight and the tensor pipe would drain after every tap.
+template <int S, int BN, int TF32, int NKS>
+__device__ __forceinline__ void halo_chunk_mma(float (&acc)[S][BN / 2], TcRing& rb, uint32_t a0, uint32_t a_sbo, int kh, int kw, int HW,
+                                               uint32_t& fresh, bool leader) {
+  using namespace tc;
+  int pend = -1;
+  for (int ky = 0; ky < kh; ++ky) {
+    for (int kx = 0; kx < kw; ++kx) {
+      mbar_wait(rb.full(), rb.ph);
+      wgmma_fence();
+      halo_tap_mma<S, BN, TF32, NKS>(acc, a0 + (uint32_t)(ky * HW + kx) * 128u, rb.slot(), a_sbo, fresh);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (pend >= 0 && leader) mbar_arrive(rb.empty0 + 8u * (uint32_t)pend);
+      pend = rb.i;
+      rb.next();
+      fresh = 1u;
+    }
+  }
+  wgmma_wait<0>();
+  if (leader) mbar_arrive(rb.empty0 + 8u * (uint32_t)pend);
+}
+
 // MMA main loop of one tile of the halo-resident kernels (conv_halo.cu, conv_chain.cu) for one consumer warpgroup: wg 0 / 1 owns
 // pixel rows 0-7 / 8-15 of every 8 x 16 sub-tile (M = 64 each).  Per (source, channel chunk) one A slot holds the HW x HH pixel
 // halo (128 B per pixel, SWIZZLE_128B); tap (ky, kx) reads it through a descriptor whose start is shifted by (ky * HW + kx) pixels
@@ -177,28 +203,13 @@ __device__ __forceinline__ void halo_tile_mma(float (&acc)[S][BN / 2], TcRing& r
       const int nks = ((rem >= chunk ? chunk : rem) * esize) >> 5;        // 32-byte K steps (16 bf16 / 8 tf32) with real channels
       mbar_wait(ra.full(), ra.ph);
       const uint32_t a0 = ra.slot() + (uint32_t)wg * 8u * a_sbo;
-      int pend = -1;
-      for (int ky = 0; ky < kh; ++ky) {
-        for (int kx = 0; kx < kw; ++kx) {
-          mbar_wait(rb.full(), rb.ph);
-          wgmma_fence();
-          const uint32_t at = a0 + (uint32_t)(ky * HW + kx) * 128u, bt = rb.slot();
-          switch (nks) {                                                   // compile-time K steps: no wgmma in a run-time loop
-            case 4: halo_tap_mma<S, BN, TF32, 4>(acc, at, bt, a_sbo, fresh); break;
-            case 3: halo_tap_mma<S, BN, TF32, 3>(acc, at, bt, a_sbo, fresh); break;
-            case 2: halo_tap_mma<S, BN, TF32, 2>(acc, at, bt, a_sbo, fresh); break;
-            default: halo_tap_mma<S, BN, TF32, 1>(acc, at, bt, a_sbo, fresh); break;
-          }
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (pend >= 0 && leader) mbar_arrive(rb.empty0 + 8u * (uint32_t)pend);
-          pend = rb.i;
-          rb.next();
-          fresh = 1u;
-        }
+      switch (nks) {                                                       // compile-time K steps: no wgmma in a run-time loop
+        case 4: halo_chunk_mma<S, BN, TF32, 4>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
+        case 3: halo_chunk_mma<S, BN, TF32, 3>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
+        case 2: halo_chunk_mma<S, BN, TF32, 2>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
+        default: halo_chunk_mma<S, BN, TF32, 1>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
       }
-      wgmma_wait<0>();
-      if (leader) { mbar_arrive(rb.empty0 + 8u * (uint32_t)pend); mbar_arrive(ra.empty()); }
+      if (leader) mbar_arrive(ra.empty());
       ra.next();
     }
   }
