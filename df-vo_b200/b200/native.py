@@ -82,6 +82,16 @@ SIGNATURES = {
     "dfvo_essential_tail": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double,
                                     c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p,
                                     c_void_p, c_void_p]),
+    "dfvo_essential_flow_tail_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "dfvo_essential_flow_tail": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double,
+                                         c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p,
+                                         c_void_p, c_void_p]),
+    "dfvo_flow_mean": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "dfvo_pnp_filter": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_void_p]),
+    "dfvo_pnp_tail_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "dfvo_pnp_tail": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_double, c_double, c_double, c_double,
+                              c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p]),
     "dfvo_epnp_minimal": (c_int, [c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double, c_int, c_void_p, c_void_p, c_void_p]),
     "dfvo_cv_subset_stream_host": (c_int, [c_int, c_int, c_int, c_void_p]),
     "dfvo_triangulate_depth": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),

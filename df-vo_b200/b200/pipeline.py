@@ -1,7 +1,8 @@
 """Device-resident DF-VO frame pipeline: uint8 frame in, 4x4 pose out.
 
 The same per-frame algorithm as the reference driver's ``deep_model_inference`` + ``tracking``
-(dfvo.py:121-262,299-345, hybrid tracking, default configuration) but organised for the GPU:
+(dfvo.py:121-262,299-345, hybrid tracking, default configuration; also ``tracking_method: PnP`` and the E-tracker's
+``validity.method: flow``) but organised for the GPU:
 everything from the uploaded frame to the keypoints / RANSAC scores / triangulated depths stays in HBM;
 the host only draws the RNG-dependent permutations, takes the small decisions the reference takes on the
 host (GRIC vote, cheirality threshold, sentinels) and chains the pose.  Per frame the host receives a few
@@ -76,6 +77,12 @@ class FramePipeline:
         thread and then waits for the pose of frame t-inflight, which that thread has been working on meanwhile: the host work
         of enqueueing a frame and the tracker's device waits overlap instead of adding up."""
         self.cfg = cfg or cfg_mod.default_cfg(height, width)
+        self.tracking_method = self.cfg.get("tracking_method", "hybrid")
+        self.validity = self.cfg.e_tracker.validity.method
+        if self.tracking_method not in ("hybrid", "PnP"):
+            raise ValueError("FramePipeline implements tracking_method 'hybrid' and 'PnP', not %r" % (self.tracking_method,))
+        if self.validity not in ("GRIC", "flow"):
+            raise ValueError("FramePipeline implements e_tracker.validity.method 'GRIC' and 'flow', not %r" % (self.validity,))
         self.K = [float(v) for v in K]
         self.H, self.W = height, width
         self.rt = runtime or rt_mod.get()
@@ -205,7 +212,7 @@ class FramePipeline:
                 self._buf("fdif%d" % slot, e.flow_diff.shape, np.float32))
 
     def track(self, cur, ref=None):
-        """dfvo.py:121-262 (hybrid).  Returns the relative pose cur -> ref as a 4x4."""
+        """dfvo.py:121-262 (tracking_method hybrid or PnP).  Returns the relative pose cur -> ref as a 4x4."""
         return self.track_finish(self.track_launch(cur, ref))
 
     def track_launch(self, cur, ref=None):
@@ -217,15 +224,29 @@ class FramePipeline:
         fwd = cur.fwd if cur.fwd is not None else eng.flow_fwd          # (subclasses may leave the flows in the engine's buffers)
         diff = cur.diff if cur.diff is not None else eng.flow_diff
         b = c.kp_selection.local_bestN
+        # flow validity on the fused path: the selection's one status read also carries the gate's mean flow magnitude
+        want_mean = self.tracking_method == "hybrid" and self.validity == "flow" and self.fused_tail
+        flow_mean = None
         if b.enable:
-            good, n, kp1_buf, kp2_buf = eng.select_local_bestn(diff, fwd, b.num_row, b.num_col, b.num_bestN, b.thre)
+            sel = eng.select_local_bestn(diff, fwd, b.num_row, b.num_col, b.num_bestN, b.thre, with_flow_mean=want_mean)
+            good, n, kp1_buf, kp2_buf = sel[:4]
+            flow_mean = sel[4] if want_mean else None
         else:
             good, n, kp1_buf, kp2_buf = eng.select_bestn(diff, fwd, c.kp_selection.bestN.num_bestN)
+            if want_mean:
+                flow_mean = eng.flow_mean(kp1_buf, kp2_buf, n)
         self.last = dict(good=good, n=n, mode="const")
         if not good:
             return dict(pose=self.motion.copy())                          # constant motion (dfvo.py:157-161)
+        if self.tracking_method == "PnP":                                 # E_pose stays identity: PnP on every frame (dfvo.py:224-250)
+            self.last["mode"] = "PnP"
+            if self.fused_tail and n <= eng.TAIL_MAX_N:
+                return dict(pnp=self.pnp_fused_launch(kp1_buf, kp2_buf, n, ref))
+            return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
         iterative = c.scale_recovery.method == "iterative"
         if not iterative and 10 < n <= eng.TAIL_MAX_N and self.fused_tail:
+            if self.validity == "flow":
+                return self.track_fused_flow_launch(cur, ref, kp1_buf, kp2_buf, n, flow_mean)
             return self.track_fused_launch(cur, ref, kp1_buf, kp2_buf, n)
         return dict(pose=self.track_stepwise(cur, ref, kp1_buf, kp2_buf, n))
 
@@ -233,6 +254,8 @@ class FramePipeline:
         """Second half of `track`: the relative pose cur -> ref (4x4)."""
         if "pose" in tok:
             return tok["pose"]
+        if "pnp" in tok:
+            return self.pnp_fused_finish(tok["pnp"])
         return self.track_fused_finish(tok)
 
     def track_stepwise(self, cur, ref, kp1_buf, kp2_buf, n):
@@ -246,7 +269,8 @@ class FramePipeline:
         # work of the scale recovery (triangulation, depth gather) is issued before the vote is joined.
         r = tracking.compute_pose_2d2d(eng, kp_ref, kp_cur, K, repeat=c.e_tracker.ransac.repeat,
                                        reproj_thre=c.e_tracker.ransac.reproj_thre, rng=self.rng,
-                                       kp_ref_buf=kp1_buf, kp_cur_buf=kp2_buf, defer_validity=True)
+                                       kp_ref_buf=kp1_buf, kp_cur_buf=kp2_buf, defer_validity=True, validity=self.validity,
+                                       flow_thre=c.e_tracker.validity.get("thre"))
         prep = None
         iterative = c.scale_recovery.method == "iterative"
         if np.linalg.norm(r["t"]) != 0 and not iterative:
@@ -288,6 +312,40 @@ class FramePipeline:
         w = eng.essential_launch(kp2_buf, kp1_buf, n, perms, K, threshold=c.e_tracker.ransac.reproj_thre)
         tail = eng.essential_tail_launch(w, h, kp2_buf, kp1_buf, n, K, cur.depth, self.rng, rs.min_samples, rs.max_trials, rs.stop_prob, rs.thre)
         return dict(tail=tail, w=w, ref=ref, kp1_buf=kp1_buf, kp2_buf=kp2_buf, n=n, last=self.last)
+
+    def track_fused_flow_launch(self, cur, ref, kp1_buf, kp2_buf, n, flow_mean):
+        """track_fused_launch for e_tracker.validity.method 'flow' (E_tracker.py:182-186,249-257): the gate on the mean flow magnitude
+        the selection read returned; a closed gate draws no shuffle and leaves E_pose at identity, so the PnP fallback runs.  Otherwise
+        the shuffles, the essential-matrix repeats and the flow-mode tail (Engine.essential_flow_tail_launch), read once by
+        track_fused_finish."""
+        c, eng, K = self.cfg, self.eng, self.K
+        self.last["flow_mean"] = flow_mean
+        if not flow_mean > c.e_tracker.validity.thre:
+            self.last.update(valid=False, inliers=np.ones(n, bool), mode="PnP", scale=None)
+            return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
+        rs = c.scale_recovery.ransac
+        perms = []
+        for _ in range(c.e_tracker.ransac.repeat):
+            order = np.arange(0, n, 1)
+            self.rng.shuffle(order)
+            perms.append(order)
+        w = eng.essential_launch(kp2_buf, kp1_buf, n, perms, K, threshold=c.e_tracker.ransac.reproj_thre)
+        tail = eng.essential_flow_tail_launch(w, kp2_buf, kp1_buf, n, K, cur.depth, self.rng, rs.min_samples, rs.max_trials, rs.stop_prob,
+                                              rs.thre)
+        return dict(tail=tail, w=w, ref=ref, kp1_buf=kp1_buf, kp2_buf=kp2_buf, n=n, last=self.last)
+
+    def pnp_fused_launch(self, kp1_buf, kp2_buf, n, ref=None):
+        """PnP tracker on the device keypoints (Engine.pnp_tail_launch): filter + unprojection, one read of the filtered count, the
+        shuffles, the solver repeats; pnp_fused_finish reads the packed result.  Same pose bits and generator stream as `pnp`."""
+        c = self.cfg
+        ref = ref or self.ref
+        pr = c.pnp_tracker.ransac
+        return self.eng.pnp_tail_launch(kp1_buf, kp2_buf, n, ref.depth, self.K, c.depth.min_depth, c.depth.max_depth, self.rng,
+                                        repeat=pr.repeat, iters=pr.iter, reproj_thre=pr.reproj_thre)
+
+    def pnp_fused_finish(self, tok):
+        pose, _, _ = self.eng.pnp_tail_finish(tok)
+        return pose
 
     def track_fused_finish(self, tok):
         eng = self.eng

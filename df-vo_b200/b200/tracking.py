@@ -104,9 +104,12 @@ class Engine:
         return raw_out, out
 
     # ------------------------------------------------------------------ selection
-    def select_local_bestn(self, diff_buf, flow_fwd_buf, rows, cols, num_bestN, thre, depth_diff_buf=None, depth_thre=0.05):
+    def select_local_bestn(self, diff_buf, flow_fwd_buf, rows, cols, num_bestN, thre, depth_diff_buf=None, depth_thre=0.05,
+                           with_flow_mean=False):
         """local_bestN (kp_selection.py:74-200) + keypoint gather.  Returns (good, n, kp1, kp2, mask-less)
-        with kp buffers float64 [num_bestN, 2] (first n rows valid).  One small D2H (status)."""
+        with kp buffers float64 [num_bestN, 2] (first n rows valid).  One small D2H (status).
+        with_flow_mean: the same single read also carries the mean flow magnitude of the selection (the E-tracker's 'flow'
+        validity gate, dfvo_flow_mean), appended as a fifth element."""
         quota = num_bestN // (rows * cols)
         key = (rows, cols, quota)
         if key not in self._sel:
@@ -119,8 +122,21 @@ class Engine:
                                                  rows, cols, num_bestN, thre, depth_thre, s["idx"].ptr, s["cc"].ptr, s["st"].ptr, st))
         self.lib.check(self.lib.dfvo_gather_keypoints(s["idx"].ptr, s["cc"].ptr, rows * cols, quota, flow_fwd_buf.ptr, self.H,
                                                       self.W, s["kp1"].ptr, s["kp2"].ptr, s["n"].ptr, st))
+        if with_flow_mean:                                        # the mean flow magnitude travels with the status (one read)
+            if "fm" not in s:
+                s["fm"] = self.rt.empty((3,), np.float64)
+            self.lib.check(self.lib.dfvo_flow_mean(s["kp1"].ptr, s["kp2"].ptr, 0, s["st"].ptr, s["fm"].ptr, st))
+            o = s["fm"].numpy()
+            return bool(o[0]), int(o[1]), s["kp1"], s["kp2"], float(o[2])
         status = s["st"].numpy()
         return bool(status[0]), int(status[1]), s["kp1"], s["kp2"]
+
+    def flow_mean(self, kp_ref_buf, kp_cur_buf, n):
+        """np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1)) of n device keypoint pairs, bit-equal to NumPy (E_tracker.py:184)."""
+        if not hasattr(self, "_fm"):
+            self._fm = self.rt.empty((3,), np.float64)
+        self.lib.check(self.lib.dfvo_flow_mean(kp_ref_buf.ptr, kp_cur_buf.ptr, int(n), None, self._fm.ptr, self.rt.stream_ptr()))
+        return float(self._fm.numpy()[2])
 
     def select_bestn(self, diff_buf, flow_fwd_buf, N):
         """bestN_flow_kp (kp_selection.py:33-71)."""
@@ -290,6 +306,84 @@ class Engine:
             out["scale"] = float(o[0])
         return out
 
+    def essential_flow_tail_launch(self, w, kp_cur_buf, kp_ref_buf, n, K, depth_buf, rng, min_samples=3, max_trials=100, stop_prob=0.99,
+                                   thre=0.1):
+        """:meth:`essential_tail_launch` for e_tracker.validity.method 'flow' (dfvo_essential_flow_tail): the per-repeat recoverPose
+        counts, the flow-mode best-E rule and vote, then the same recoverPose / cheirality gate / scale recovery.  The caller took the
+        flow gate before drawing the shuffles of `w`.  depth_buf None: pose only (no scale recovery, `rng` untouched).  Finish with
+        :meth:`essential_tail_finish`; its E_gric holds the per-repeat cheirality counts, H_gric is 0."""
+        cx, cy, fx, fy = K
+        R = w["info"].shape[0]
+        cap = w["cap"]
+        c = getattr(self, "_ftail", None)
+        if c is None or c["cap"] < cap or c["R"] != R:
+            nb = int(self.lib.dfvo_essential_flow_tail_workspace_bytes(cap, R))
+            c = self._ftail = dict(cap=cap, R=R, ws=self.rt.empty((nb,), np.uint8), res=self.rt.empty((335 + 5 * R,), np.float64),
+                                   host=np.zeros(335 + 5 * R, np.float64))
+        st = rng.get_state()
+        if st[0] != "MT19937":
+            raise TypeError("essential_flow_tail needs a legacy MT19937 generator (np.random / np.random.RandomState)")
+        u = c["host"][4:317].view(np.uint32)
+        u[:624] = st[1]
+        u[624] = st[2]
+        c["res"].upload(c["host"])
+        self.lib.check(self.lib.dfvo_essential_flow_tail(w["E"].ptr, w["info"].ptr, R, kp_cur_buf.ptr, kp_ref_buf.ptr, n, fx, fy, cx, cy,
+                                                         depth_buf.ptr if depth_buf is not None else None, self.H, self.W,
+                                                         int(min_samples), int(max_trials), float(stop_prob), float(thre), c["ws"].ptr,
+                                                         c["ws"].shape[0], c["res"].ptr, w["pmask"].ptr, w["pinfo"].ptr,
+                                                         self.rt.stream_ptr()))
+        return dict(c=c, w=w, n=n, R=R, rng=rng, st=st)
+
+    def pnp_tail_launch(self, kp_ref_buf, kp_cur_buf, n, depth_buf, K, min_depth, max_depth, rng, repeat=5, iters=100, reproj_thre=1.0,
+                        prob=0.99):
+        """``PnpTracker.compute_pose_3d2d`` (pnp_tracker.py:45-125) on device keypoints: dfvo_pnp_filter (in-image filter, reference depth
+        at int(kp_ref), depth range, ordered compaction, unprojection), ONE read of the filtered count m, the host's `repeat` shuffles of
+        arange(m) (drawn even when m <= 4, as the reference does), then dfvo_pnp_tail (the solvePnPRansac repeats and the best one).
+        Finish with :meth:`pnp_tail_finish` (one packed read)."""
+        cx, cy, fx, fy = K
+        if not hasattr(self, "_pf") or self._pf["cap"] < n:
+            cap = self._capacity(n)
+            self._pf = dict(cap=cap, obj=self.rt.empty((cap * 3,), np.float64), img=self.rt.empty((cap * 2,), np.float64),
+                            m=self.rt.empty((1,), np.int32))
+        f = self._pf
+        iK = np.ascontiguousarray(np.linalg.inv(np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1.0]])))    # as compute_pose_3d2d unprojects
+        self.lib.check(self.lib.dfvo_pnp_filter(kp_ref_buf.ptr, kp_cur_buf.ptr, n, depth_buf.ptr, self.H, self.W, float(min_depth),
+                                                float(max_depth), iK.ctypes.data_as(ctypes.c_void_p), f["obj"].ptr, f["img"].ptr,
+                                                f["m"].ptr, self.rt.stream_ptr()))
+        m = int(f["m"].numpy()[0])                                        # the one read before the solver
+        perms = []
+        for _ in range(repeat):                                           # pnp_tracker.py:90-95
+            order = np.arange(0, m, 1)
+            rng.shuffle(order)
+            perms.append(order)
+        if m <= 4:                                                        # pnp_tracker.py:97: no solver, identity
+            return dict(m=m, res=None)
+        key = (repeat, iters)
+        c = self._pnp_ws.get(("tail",) + key)
+        if c is None or c["cap"] < m:
+            cap = self._capacity(m)
+            nb = int(self.lib.dfvo_pnp_tail_workspace_bytes(cap, repeat, iters))
+            c = self._pnp_ws[("tail",) + key] = dict(cap=cap, ws=self.rt.empty((nb,), np.uint8), perm_c=self.rt.empty((repeat * cap,), np.int32),
+                                                     res=self.rt.empty((8 + 4 * repeat,), np.float64))
+        perm = c["perm_c"].view((repeat, m)).upload(np.asarray(perms, np.int32))
+        self.lib.check(self.lib.dfvo_pnp_tail(f["obj"].ptr, f["img"].ptr, m, perm.ptr, repeat, self._subset_table(m, iters).ptr, iters,
+                                              fx, fy, cx, cy, float(reproj_thre), prob, c["ws"].ptr, c["ws"].shape[0], c["res"].ptr,
+                                              self.rt.stream_ptr()))
+        return dict(m=m, res=c["res"])
+
+    def pnp_tail_finish(self, tok):
+        """-> (4x4 pose current -> reference, winning inlier count, filtered count).  The pose is assembled exactly as
+        :func:`compute_pose_3d2d` does it (hostmath.rodrigues, np.linalg.inv), so both paths give the same bits."""
+        pose = np.eye(4)
+        best_inl = 0
+        if tok["res"] is not None:
+            o = tok["res"].numpy()                                        # the one packed read
+            if o[0] >= 0:
+                best_inl = int(o[1])
+                pose[:3, :3] = hostmath.rodrigues(o[2:5].copy())
+                pose[:3, 3] = o[5:8]
+        return np.linalg.inv(pose), best_inl, tok["m"]
+
     def recover_pose(self, w, best, kp_cur_buf, kp_ref_buf, n, K):
         """cv2.recoverPose(best_E, kp_cur, kp_ref, focal=fx, pp) (E_tracker.py:292-295)."""
         cx, cy, fx, fy = K
@@ -389,8 +483,9 @@ class Engine:
 # host-level orchestration of the E-tracker (E_tracker.py:154-307, validity.method == 'GRIC')
 # ---------------------------------------------------------------------------------------------
 def compute_pose_2d2d(engine, kp_ref, kp_cur, K, repeat=5, reproj_thre=0.2, rng=np.random, kp_ref_buf=None, kp_cur_buf=None,
-                      defer_validity=False):
-    """Same contract as ``EssTracker.compute_pose_2d2d`` with the default GRIC validity check.
+                      defer_validity=False, validity="GRIC", flow_thre=None):
+    """Same contract as ``EssTracker.compute_pose_2d2d`` with the default GRIC validity check (validity='flow': the flow-magnitude
+    check with threshold `flow_thre`, see :func:`_compute_pose_2d2d_flow`).
     kp_ref/kp_cur: float64 [N,2] host arrays (device copies optional).  Everything numeric runs on the device: the
     homography model + GRIC-H (csrc/homog.cu), the five essential-matrix RANSAC repeats + GRIC-E (ransac.cu) and
     recoverPose; the host draws the shuffles, takes the majority vote and the cheirality decision.
@@ -402,6 +497,8 @@ def compute_pose_2d2d(engine, kp_ref, kp_cur, K, repeat=5, reproj_thre=0.2, rng=
     n = kp_ref.shape[0]
     R, t = np.eye(3), np.zeros((3, 1))
     out = dict(R=R, t=t, inliers=np.ones(n, bool), valid=False, cheirality=0)
+    if validity == "flow":
+        return _compute_pose_2d2d_flow(engine, kp_ref, kp_cur, K, repeat, reproj_thre, rng, kp_ref_buf, kp_cur_buf, flow_thre, out)
     if n <= 10:                                                     # E_tracker.py:196,216-217
         return out
     # host RNG consumption identical to the reference: one shuffle per repeat (E_tracker.py:225-226)
@@ -432,6 +529,32 @@ def compute_pose_2d2d(engine, kp_ref, kp_cur, K, repeat=5, reproj_thre=0.2, rng=
     out["_vote"] = (h, gric, repeat, best)
     if not defer_validity:
         resolve_validity(out)
+    return out
+
+
+def _compute_pose_2d2d_flow(engine, kp_ref, kp_cur, K, repeat, reproj_thre, rng, kp_ref_buf, kp_cur_buf, flow_thre, out):
+    """E_tracker.py:182-186,249-257,289-300 (validity.method 'flow'): the gate mean |kp_ref - kp_cur| > thre is NumPy's own expression
+    on the host arrays; a closed gate draws no shuffle and leaves the pose at identity.  Otherwise the repeats, the per-repeat
+    recoverPose counts, the flow-mode best-E rule, the vote and the final recoverPose run on the device (essential_ransac +
+    dfvo_essential_flow_tail without scale recovery) and are read once."""
+    n = kp_ref.shape[0]
+    avg_flow = np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1))
+    out["flow_mean"] = avg_flow
+    if not avg_flow > flow_thre:
+        return out
+    perms = []
+    for _ in range(repeat):
+        order = np.arange(0, n, 1)
+        rng.shuffle(order)
+        perms.append(order)
+    rt = engine.rt
+    kp_cur_buf = kp_cur_buf or rt.from_host(kp_cur)
+    kp_ref_buf = kp_ref_buf or rt.from_host(kp_ref)
+    w = engine.essential_launch(kp_cur_buf, kp_ref_buf, n, perms, K, threshold=reproj_thre)
+    o = engine.essential_tail_finish(engine.essential_flow_tail_launch(w, kp_cur_buf, kp_ref_buf, n, K, None, rng))
+    out.update(valid=o["valid"], cheirality=o["cheirality"], R=o["R"], t=o["t"], ransac_info=o["ransac_info"], cheirality_counts=o["E_gric"])
+    if o["best"] >= 0:
+        out["inliers"] = w["mask"].numpy()[o["best"]].astype(bool)
     return out
 
 

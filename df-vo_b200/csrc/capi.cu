@@ -573,6 +573,41 @@ int dfvo_essential_tail(const double* E, const int32_t* info, const double* gric
   API_END
 }
 
+size_t dfvo_essential_flow_tail_workspace_bytes(int N, int R) { return essential_flow_tail_workspace_bytes(N, R); }
+int dfvo_essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx,
+                             double fy, double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials,
+                             double stop_prob, double threshold, void* workspace, size_t workspace_bytes, double* res, uint8_t* pose_mask,
+                             int32_t* pose_info, void* stream) {
+  API_BEGIN
+  return essential_flow_tail(E, info, R, kp_cur, kp_ref, N, fx, fy, cx, cy, depth, H, W, min_samples, max_trials, stop_prob, threshold,
+                             workspace, workspace_bytes, res, pose_mask, pose_info, (cudaStream_t)stream);
+  API_END
+}
+
+int dfvo_flow_mean(const double* kp_ref, const double* kp_cur, int n, const int32_t* status, double* out, void* stream) {
+  API_BEGIN
+  DFVO_REQUIRE(kp_ref && kp_cur && out, DFVO_EINVAL, "dfvo_flow_mean args");
+  return flow_mean(kp_ref, kp_cur, n, status, out, (cudaStream_t)stream);
+  API_END
+}
+
+int dfvo_pnp_filter(const double* kp_ref, const double* kp_cur, int n, const float* depth, int H, int W, double min_depth, double max_depth,
+                    const double* iK_host, double* obj, double* img, int32_t* count, void* stream) {
+  API_BEGIN
+  return pnp_filter(kp_ref, kp_cur, n, depth, H, W, min_depth, max_depth, iK_host, obj, img, count, (cudaStream_t)stream);
+  API_END
+}
+
+size_t dfvo_pnp_tail_workspace_bytes(int N, int R, int iters) { return pnp_tail_workspace_bytes(N, R, iters); }
+int dfvo_pnp_tail(const double* obj, const double* img, int N, const int32_t* perm, int R, const int32_t* subsets, int iters, double fx,
+                  double fy, double cx, double cy, double threshold, double prob, void* workspace, size_t workspace_bytes, double* res,
+                  void* stream) {
+  API_BEGIN
+  DFVO_REQUIRE(workspace != nullptr, DFVO_EINVAL, "dfvo_pnp_tail: null workspace");
+  return pnp_tail(obj, img, N, perm, R, subsets, iters, fx, fy, cx, cy, threshold, prob, workspace, workspace_bytes, res, (cudaStream_t)stream);
+  API_END
+}
+
 int dfvo_epnp_minimal(const double* obj, const double* img, int M, double fx, double fy, double cx, double cy, int coop, double* rt,
                       int32_t* ok, void* stream) {
   API_BEGIN

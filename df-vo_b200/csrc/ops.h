@@ -164,6 +164,9 @@ int uniform_cells(const float* rigid_diff, const float* flow_diff, int H, int W,
 int rigid_flow_diff(const float* depth, const float* flow, int H, int W, const double* T_host, double fx, double fy, double cx, double cy,
                     float* out, cudaStream_t s);
 int gather_depth(const float* depth, int H, int W, const double* kp, int n, float* out, cudaStream_t s);
+// np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1)) bit for bit; status (local_bestn's, nullable) supplies good / n on the device.
+// out [3] = {good, n, mean}
+int flow_mean(const double* kp_ref, const double* kp_cur, int n, const int32_t* status, double* out, cudaStream_t s);
 
 // ---- geometry layers (geometry.cu): libs/geometry/{backprojection,transformation3d,projection,reprojection,rigid_flow}.py ----
 // host matrices are row-major float64 (cast to float32 like torch.from_numpy(..).float()); points are planar [4][H*W]

@@ -787,4 +787,85 @@ int pnp_ransac(const double* obj, const double* img, int N, const int32_t* perm,
   return DFVO_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Fused PnP tracker (pnp_tracker.py:45-125), in two enqueues around the one value the host needs -- the filtered count, which sizes
+// the shuffles and picks OpenCV's subset stream:
+//   pnp_filter  keypoints whose kp_cur lies inside the image, reference depth at int(kp_ref), 0 < min < d < max, compacted in order,
+//               unprojected (ops_3d.py:70-94): X = (iK00 u + iK02) d, Y = (iK11 v + iK12) d, Z = d -- the rounding of NumPy's
+//               (inv(K) @ [u v 1]^T) * d, whose zero entries of inv(K) add nothing
+//   pnp_tail    the R solvePnPRansac repeats of pnp_ransac, then the first repeat with the most inliers (found && inliers > best)
+// ------------------------------------------------------------------------------------------------
+#define PF_THREADS 1024
+__global__ void __launch_bounds__(PF_THREADS)
+k_pnp_filter(const double* __restrict__ kp_ref, const double* __restrict__ kp_cur, int n, const float* __restrict__ depth, int H, int W,
+             double min_depth, double max_depth, double ik00, double ik02, double ik11, double ik12, double* __restrict__ obj,
+             double* __restrict__ img, int32_t* __restrict__ count) {
+  __shared__ int wsum[PF_THREADS / 32];
+  const int t = threadIdx.x;
+  const int chunk = (n + PF_THREADS - 1) / PF_THREADS;
+  const int i0 = t * chunk < n ? t * chunk : n, i1 = i0 + chunk < n ? i0 + chunk : n;
+  auto depth_of = [&](int i, double* d) -> bool {
+    const double u2 = kp_cur[2 * i], v2 = kp_cur[2 * i + 1];
+    if (!(u2 >= 0 && u2 < W && v2 >= 0 && v2 < H)) return false;
+    const int x = (int)kp_ref[2 * i], y = (int)kp_ref[2 * i + 1];
+    *d = (x >= 0 && x < W && y >= 0 && y < H) ? (double)depth[(size_t)y * W + x] : 0.0;
+    return *d != 0 && *d < max_depth && *d > min_depth;
+  };
+  int cnt = 0;
+  double d;
+  for (int i = i0; i < i1; ++i) cnt += depth_of(i, &d) ? 1 : 0;
+  int incl = cnt;
+  for (int off = 1; off < 32; off <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, off); if ((t & 31) >= off) incl += v; }
+  if ((t & 31) == 31) wsum[t >> 5] = incl;
+  __syncthreads();
+  if (t == 0) { int a = 0; for (int w8 = 0; w8 < PF_THREADS / 32; ++w8) { const int v = wsum[w8]; wsum[w8] = a; a += v; } *count = a; }
+  __syncthreads();
+  int o = wsum[t >> 5] + incl - cnt;
+  for (int i = i0; i < i1; ++i) {
+    if (!depth_of(i, &d)) continue;
+    obj[3 * o] = __dmul_rn(__dadd_rn(__dmul_rn(ik00, kp_ref[2 * i]), ik02), d);
+    obj[3 * o + 1] = __dmul_rn(__dadd_rn(__dmul_rn(ik11, kp_ref[2 * i + 1]), ik12), d);
+    obj[3 * o + 2] = d;
+    img[2 * o] = kp_cur[2 * i];
+    img[2 * o + 1] = kp_cur[2 * i + 1];
+    ++o;
+  }
+}
+
+int pnp_filter(const double* kp_ref, const double* kp_cur, int n, const float* depth, int H, int W, double min_depth, double max_depth,
+               const double* iK, double* obj, double* img, int32_t* count, cudaStream_t s) {
+  DFVO_REQUIRE(kp_ref && kp_cur && depth && iK && obj && img && count && n >= 1 && H > 0 && W > 0, DFVO_EINVAL, "pnp_filter args (n=%d)", n);
+  DFVO_REQUIRE(iK[1] == 0.0 && iK[3] == 0.0 && iK[6] == 0.0 && iK[7] == 0.0 && iK[8] == 1.0, DFVO_EINVAL, "pnp_filter: iK is not inv([[fx,0,cx],[0,fy,cy],[0,0,1]])");
+  DFVO_LAUNCH(k_pnp_filter, dim3(1), dim3(PF_THREADS), 0, s, kp_ref, kp_cur, n, depth, H, W, min_depth, max_depth, iK[0], iK[2], iK[4], iK[5],
+              obj, img, count);
+  DFVO_CHECK_LAUNCH();
+  return DFVO_OK;
+}
+
+__global__ void k_pnp_pick(const double* __restrict__ rt, const int32_t* __restrict__ info, int R, double* __restrict__ res) {
+  if (threadIdx.x != 0) return;
+  int best = -1, best_inl = 0;
+  for (int r = 0; r < R; ++r)
+    if (info[4 * r] && info[4 * r + 1] > best_inl) { best = r; best_inl = info[4 * r + 1]; }   // pnp_tracker.py:108-110
+  res[0] = (double)best;
+  res[1] = (double)best_inl;
+  for (int k = 0; k < 6; ++k) res[2 + k] = best >= 0 ? rt[6 * best + k] : 0.0;
+  for (int q = 0; q < 4 * R; ++q) res[8 + q] = (double)info[q];
+}
+
+size_t pnp_tail_workspace_bytes(int N, int R, int iters) { return pnp_workspace_bytes(N, R, iters) + (size_t)R * (6 * 8 + 4 * 4) + 256; }
+
+int pnp_tail(const double* obj, const double* img, int N, const int32_t* perm, int R, const int32_t* subsets, int iters, double fx, double fy,
+             double cx, double cy, double threshold, double prob, void* workspace, size_t ws_bytes, double* res, cudaStream_t s) {
+  DFVO_REQUIRE(res != nullptr && ws_bytes >= pnp_tail_workspace_bytes(N, R, iters), DFVO_EINVAL, "pnp_tail workspace too small");
+  uint8_t* w = reinterpret_cast<uint8_t*>(workspace);
+  const size_t head = (pnp_workspace_bytes(N, R, iters) + 127) & ~(size_t)127;
+  double* rt = (double*)(w + head);
+  int32_t* info = (int32_t*)(w + head + (((size_t)R * 6 * 8 + 127) & ~(size_t)127));
+  { const int rc = pnp_ransac(obj, img, N, perm, R, subsets, iters, fx, fy, cx, cy, threshold, prob, workspace, head, rt, info, s); if (rc) return rc; }
+  DFVO_LAUNCH(k_pnp_pick, dim3(1), dim3(32), 0, s, (const double*)rt, (const int32_t*)info, R, res);
+  DFVO_CHECK_LAUNCH();
+  return DFVO_OK;
+}
+
 }  // namespace dfvo

@@ -399,6 +399,23 @@ DFVO_D void decompose_essential(const double* __restrict__ Eptr, double R[2][3][
   for (int i = 0; i < 3; ++i) tv[i] = U[i][2];
 }
 
+// Cheirality test of point j under candidate k (recoverPose's triangulate + depth checks).
+DFVO_D bool cheirality_ok(const double (*sR)[3][3], const double* st, int k, const double* __restrict__ p1, const double* __restrict__ p2,
+                          int j, double focal, double cx, double cy, double dist) {
+  const double u0 = (p1[2 * j] - cx) / focal, v0 = (p1[2 * j + 1] - cy) / focal;
+  const double u1 = (p2[2 * j] - cx) / focal, v1 = (p2[2 * j + 1] - cy) / focal;
+  double P[3][4];
+  const double sg = k < 2 ? 1.0 : -1.0;
+  for (int a = 0; a < 3; ++a) { for (int b = 0; b < 3; ++b) P[a][b] = sR[k & 1][a][b]; P[a][3] = sg * st[a]; }
+  double X[4];
+  triangulate_dlt(P, u0, v0, u1, v1, X);
+  bool m = (X[2] * X[3]) > 0;
+  const double x = X[0] / X[3], y = X[1] / X[3], z = X[2] / X[3];
+  m = m && (z < dist);
+  const double z2 = P[2][0] * x + P[2][1] * y + P[2][2] * z + P[2][3];
+  return m && (z2 > 0) && (z2 < dist);
+}
+
 // Pass 1: one thread per (point, candidate) -- the 4 candidates of a point sit in adjacent lanes.  Every block
 // repeats the (tiny) decomposition instead of waiting for a producer kernel.  mask_out[j] receives the 4-bit
 // candidate field, info[1+k] the cheirality count of candidate k (atomics; info zeroed by the caller).
@@ -412,21 +429,7 @@ k_recover_pose_vote(const double* __restrict__ Eptr, const double* __restrict__ 
   if (t < 4) cnt[t] = 0;
   __syncthreads();
   const int g = blockIdx.x * 256 + t, j = g >> 2, k = g & 3;
-  bool m = false;
-  if (j < N) {
-    const double u0 = (p1[2 * j] - cx) / focal, v0 = (p1[2 * j + 1] - cy) / focal;
-    const double u1 = (p2[2 * j] - cx) / focal, v1 = (p2[2 * j + 1] - cy) / focal;
-    double P[3][4];
-    const double sg = k < 2 ? 1.0 : -1.0;
-    for (int a = 0; a < 3; ++a) { for (int b = 0; b < 3; ++b) P[a][b] = sR[k & 1][a][b]; P[a][3] = sg * st[a]; }
-    double X[4];
-    triangulate_dlt(P, u0, v0, u1, v1, X);
-    m = (X[2] * X[3]) > 0;
-    const double x = X[0] / X[3], y = X[1] / X[3], z = X[2] / X[3];
-    m = m && (z < dist);
-    const double z2 = P[2][0] * x + P[2][1] * y + P[2][2] * z + P[2][3];
-    m = m && (z2 > 0) && (z2 < dist);
-  }
+  const bool m = j < N && cheirality_ok(sR, st, k, p1, p2, j, focal, cx, cy, dist);
   const unsigned ballot = __ballot_sync(0xffffffffu, m);
   const int lane = t & 31;
   if (j < N && k == 0) mask_out[j] = (uint8_t)((ballot >> lane) & 0xfu);
@@ -851,6 +854,107 @@ int essential_tail(const double* E, const int32_t* info, const double* gric, int
   DFVO_LAUNCH(k_scale_chain, dim3(1), dim3(SC_THREADS), 0, s, (const unsigned long long*)keys, N, res, (const double*)zbuf, (const double*)dbuf, ratio);
   DFVO_LAUNCH(k_scale_ransac, dim3(1), dim3(SR_THREADS), 0, s, (const double*)ratio, N, min_samples, max_trials, stop_prob, thr, res, perm,
               (const double*)(res + TR_NVALID), (const double*)(res + TR_GATE));
+  DFVO_CHECK_LAUNCH();
+  return DFVO_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// The same tail for the flow-magnitude validity check (e_tracker.validity.method 'flow', E_tracker.py:249-257,289-300).  The caller has
+// already taken the gate (mean flow > thre) and drawn the shuffles only when it passed.  Per repeat r:
+//   cnt_r   = cv2.recoverPose(E_r, kp_cur[perm_r], kp_ref[perm_r]).count -- a count over all points, so the permutation drops out
+//   valid_r = cnt_r > 0.1 n;   E_r becomes the best only if inliers_r > best inliers AND cnt_r > 0.05 n
+// then the majority vote sum(valid_r) > R / 2, the final recoverPose on the best E, the cheirality gate and (depth != NULL) the scale
+// chain of essential_tail.  res layout as essential_tail's, except [319] = 0 and [335..335+R) = cnt_r.
+// ------------------------------------------------------------------------------------------------
+// every repeat's four candidate counts in one launch: grid (cdiv(4N, 256), R), counts [R][4] zeroed by the caller
+__global__ void __launch_bounds__(256)
+k_recover_pose_counts(const double* __restrict__ E, const double* __restrict__ p1, const double* __restrict__ p2, int N, double focal,
+                      double cx, double cy, double dist, int32_t* __restrict__ counts) {
+  __shared__ double sR[2][3][3], st[3];
+  __shared__ int cnt[4];
+  const int t = threadIdx.x, r = blockIdx.y;
+  if (t == 0) decompose_essential(E + 9 * r, sR, st);
+  if (t < 4) cnt[t] = 0;
+  __syncthreads();
+  const int g = blockIdx.x * 256 + t, j = g >> 2, k = g & 3;
+  const bool m = j < N && cheirality_ok(sR, st, k, p1, p2, j, focal, cx, cy, dist);
+  const unsigned ballot = __ballot_sync(0xffffffffu, m);
+  const int lane = t & 31;
+  if (lane < 4) {
+    const int c = __popc(ballot & (0x11111111u << lane));
+    if (c) atomicAdd(&cnt[lane], c);
+  }
+  __syncthreads();
+  if (t < 4 && cnt[t]) atomicAdd(&counts[4 * r + t], cnt[t]);
+}
+
+__global__ void k_track_pick_flow(const int32_t* __restrict__ info, const int32_t* __restrict__ counts, const double* __restrict__ E, int R,
+                                  int n, double* __restrict__ res, double* __restrict__ E_best) {
+  if (threadIdx.x != 0) return;
+  int best = -1, best_inl = 0, votes = 0;
+  for (int r = 0; r < R; ++r) {
+    int b = 0;                                                         // recoverPose keeps the first candidate with the most points
+    for (int k = 1; k < 4; ++k) if (counts[4 * r + k] > counts[4 * r + b]) b = k;
+    const int c = counts[4 * r + b];
+    votes += ((double)c > (double)n * 0.1) ? 1 : 0;
+    if (info[4 * r] > best_inl && (double)c > (double)n * 0.05) { best = r; best_inl = info[4 * r]; }
+    res[TR_EGRIC + r] = (double)c;
+    for (int q = 0; q < 4; ++q) res[TR_EGRIC + R + 4 * r + q] = (double)info[4 * r + q];
+  }
+  res[TR_BEST] = (double)best;
+  res[TR_VALID] = ((double)votes > (double)R / 2.0) ? 1.0 : 0.0;
+  for (int q = 0; q < 9; ++q) E_best[q] = best >= 0 ? E[9 * best + q] : ((q % 4 == 0 && q < 8) ? 1.0 : 0.0);
+}
+
+// k_track_gate with the vote already in res[TR_VALID]
+__global__ void k_track_gate_flow(double* __restrict__ res, const int32_t* __restrict__ pinfo, int n, double* __restrict__ T21) {
+  if (threadIdx.x != 0) return;
+  const bool valid = res[TR_VALID] != 0.0;
+  const int best = (int)res[TR_BEST], cheir = best >= 0 ? pinfo[0] : 0;
+  const double* Rt = res + TR_RT;
+  const bool pose_ok = valid && best >= 0 && (double)cheir > (double)n * 0.1;
+  const double tn = Rt[9] * Rt[9] + Rt[10] * Rt[10] + Rt[11] * Rt[11];
+  res[TR_HGRIC] = 0.0; res[TR_CHEIR] = (double)cheir; res[TR_GATE] = (pose_ok && tn != 0.0) ? 1.0 : 0.0; res[TR_NVALID] = 0.0;
+  for (int a = 0; a < 3; ++a) {
+    double tt = 0;
+    for (int b = 0; b < 3; ++b) { T21[4 * a + b] = Rt[3 * b + a]; tt += Rt[3 * b + a] * Rt[9 + b]; }
+    T21[4 * a + 3] = -tt;
+  }
+}
+
+size_t essential_flow_tail_workspace_bytes(int N, int R) { return essential_tail_workspace_bytes(N) + (size_t)R * 16 + 128; }
+
+int essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx, double fy,
+                        double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials, double stop_prob, double thr,
+                        void* workspace, size_t ws_bytes, double* res, uint8_t* pose_mask, int32_t* pose_info, cudaStream_t s) {
+  DFVO_REQUIRE(E && info && kp_cur && kp_ref && workspace && res && pose_mask && pose_info, DFVO_EINVAL, "essential_flow_tail args");
+  DFVO_REQUIRE(R >= 1 && R <= 32 && N >= 1 && N <= SC_MAX && min_samples >= 1 && min_samples <= SR_MAX_SAMPLES, DFVO_EINVAL,
+               "essential_flow_tail: R=%d N=%d", R, N);
+  DFVO_REQUIRE(ws_bytes >= essential_flow_tail_workspace_bytes(N, R), DFVO_EINVAL, "essential_flow_tail workspace too small");
+  uint8_t* w = reinterpret_cast<uint8_t*>(workspace);
+  auto take = [&](size_t bytes) { uint8_t* p = w; w += (bytes + 127) & ~(size_t)127; return p; };
+  double* zbuf = (double*)take((size_t)N * 8);
+  double* dbuf = (double*)take((size_t)N * 8);
+  double* ratio = (double*)take((size_t)N * 8);
+  int32_t* perm = (int32_t*)take((size_t)N * 4);
+  unsigned long long* keys = (unsigned long long*)take((size_t)N * 8);
+  double* E_best = (double*)take(9 * 8);
+  double* T21 = (double*)take(12 * 8);
+  int32_t* counts = (int32_t*)take((size_t)R * 16);
+  DFVO_CUDA(cudaMemsetAsync(counts, 0, (size_t)R * 16, s));
+  DFVO_LAUNCH(k_recover_pose_counts, dim3(cdiv(4 * N, 256), R), dim3(256), 0, s, E, kp_cur, kp_ref, N, fx, cx, cy, 50.0, counts);
+  DFVO_LAUNCH(k_track_pick_flow, dim3(1), dim3(32), 0, s, info, (const int32_t*)counts, E, R, N, res, E_best);
+  DFVO_CUDA(cudaMemsetAsync(pose_info, 0, 5 * sizeof(int32_t), s));
+  DFVO_LAUNCH(k_recover_pose_vote, dim3(cdiv(4 * N, 256)), dim3(256), 0, s, (const double*)E_best, kp_cur, kp_ref, N, fx, cx, cy, 50.0, pose_mask, pose_info);
+  DFVO_LAUNCH(k_recover_pose_pick, dim3(cdiv(N, 256)), dim3(256), 0, s, (const double*)E_best, N, res + TR_RT, pose_mask, pose_info);
+  DFVO_LAUNCH(k_track_gate_flow, dim3(1), dim3(32), 0, s, res, (const int32_t*)pose_info, N, T21);
+  if (depth != nullptr) {
+    DFVO_LAUNCH(k_scale_points, dim3(cdiv(N, 128)), dim3(128), 0, s, kp_ref, kp_cur, N, fx, fy, cx, cy, (const double*)T21, depth, H, W,
+                (const double*)res, zbuf, dbuf, keys);
+    DFVO_LAUNCH(k_scale_chain, dim3(1), dim3(SC_THREADS), 0, s, (const unsigned long long*)keys, N, res, (const double*)zbuf, (const double*)dbuf, ratio);
+    DFVO_LAUNCH(k_scale_ransac, dim3(1), dim3(SR_THREADS), 0, s, (const double*)ratio, N, min_samples, max_trials, stop_prob, thr, res, perm,
+                (const double*)(res + TR_NVALID), (const double*)(res + TR_GATE));
+  }
   DFVO_CHECK_LAUNCH();
   return DFVO_OK;
 }

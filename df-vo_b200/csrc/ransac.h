@@ -40,6 +40,21 @@ int essential_tail(const double* E, const int32_t* info, const double* gric, int
                    double fx, double fy, double cx, double cy, const double* h_gric, const float* depth, int H, int W, int min_samples,
                    int max_trials, double stop_prob, double thr, void* workspace, size_t ws_bytes, double* res, uint8_t* pose_mask,
                    int32_t* pose_info, cudaStream_t s);
+// the same tail for e_tracker.validity.method 'flow': per-repeat recoverPose counts, the flow-mode best-E rule and vote, then as above
+// (depth == nullptr: no scale recovery).  res layout as essential_tail's with [335..335+R) = per-repeat cheirality counts.
+size_t essential_flow_tail_workspace_bytes(int N, int R);
+int essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx, double fy,
+                        double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials, double stop_prob, double thr,
+                        void* workspace, size_t ws_bytes, double* res, uint8_t* pose_mask, int32_t* pose_info, cudaStream_t s);
+
+// fused PnP tracker (pnp.cu): in-image / depth-range filter + order-preserving compaction + unprojection -> obj [m][3], img [m][2],
+// count [1] = m; iK = inv(K) row-major [9] (host memory)
+int pnp_filter(const double* kp_ref, const double* kp_cur, int n, const float* depth, int H, int W, double min_depth, double max_depth,
+               const double* iK, double* obj, double* img, int32_t* count, cudaStream_t s);
+// pnp_ransac + best repeat: res [8 + 4 R] = {best, inliers, rvec, tvec, info [R][4]}
+size_t pnp_tail_workspace_bytes(int N, int R, int iters);
+int pnp_tail(const double* obj, const double* img, int N, const int32_t* perm, int R, const int32_t* subsets, int iters, double fx, double fy,
+             double cx, double cy, double threshold, double prob, void* workspace, size_t ws_bytes, double* res, cudaStream_t s);
 
 // stage entry: EPnP (cv2.solvePnP(flags=SOLVEPNP_EPNP) as solvePnPRansac's minimal solver uses it) on M independent 5-point
 // samples; coop: 1 = lane-cooperative kernel, 0 = one thread per sample, -1 = the default of the build

@@ -419,6 +419,86 @@ int gather_depth(const float* depth, int H, int W, const double* kp, int n, floa
   return DFVO_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Flow-magnitude validity (E_tracker.py:182-185): np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1)) bit for bit.  The norm of a row
+// is sqrt(dx*dx + dy*dy) with every operation rounded (no FMA); the mean is NumPy's pairwise sum (pairwise_sum in
+// loops_utils.h.src: blocks of <= 128 elements summed with 8 accumulators, larger ranges split at n/2 rounded down to a multiple
+// of 8) divided by n.  One block: the blocks of the recursion ("leaves") are summed in parallel, thread 0 adds them up in the
+// recursion's order.  Leaves hold 64..128 elements, so FM_MAX_LEAVES covers n <= FM_MAX_N.
+// ------------------------------------------------------------------------------------------------
+#define FM_THREADS 256
+#define FM_MAX_LEAVES 1200
+#define FM_MAX_N 65536
+
+DFVO_D double kp_disp(const double* __restrict__ a, const double* __restrict__ b, int i) {
+  const double dx = __dsub_rn(a[2 * i], b[2 * i]), dy = __dsub_rn(a[2 * i + 1], b[2 * i + 1]);
+  return sqrt(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
+}
+
+// pairwise_sum's base case on [lo, lo + n), n <= 128
+DFVO_D double pw_leaf(const double* __restrict__ a, const double* __restrict__ b, int lo, int n) {
+  if (n < 8) {
+    double r = 0.0;
+    for (int i = 0; i < n; ++i) r = __dadd_rn(r, kp_disp(a, b, lo + i));
+    return r;
+  }
+  double r[8];
+  for (int j = 0; j < 8; ++j) r[j] = kp_disp(a, b, lo + j);
+  int i = 8;
+  for (; i < n - (n % 8); i += 8)
+    for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], kp_disp(a, b, lo + i + j));
+  double res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])), __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
+  for (; i < n; ++i) res = __dadd_rn(res, kp_disp(a, b, lo + i));
+  return res;
+}
+
+// the leaves of pairwise_sum(lo, n) in recursion order
+DFVO_D void pw_leaves(int lo, int n, int* leaf_lo, int* leaf_n, int* count) {
+  if (n <= 128) { leaf_lo[*count] = lo; leaf_n[*count] = n; ++*count; return; }
+  int n2 = n / 2;
+  n2 -= n2 % 8;
+  pw_leaves(lo, n2, leaf_lo, leaf_n, count);
+  pw_leaves(lo + n2, n - n2, leaf_lo, leaf_n, count);
+}
+
+DFVO_D double pw_combine(int n, const double* leaf_sum, int* next) {
+  if (n <= 128) return leaf_sum[(*next)++];
+  int n2 = n / 2;
+  n2 -= n2 % 8;
+  const double l = pw_combine(n2, leaf_sum, next);
+  return __dadd_rn(l, pw_combine(n - n2, leaf_sum, next));
+}
+
+__global__ void __launch_bounds__(FM_THREADS)
+k_flow_mean(const double* __restrict__ kp_ref, const double* __restrict__ kp_cur, int n_in, const int32_t* __restrict__ status,
+            double* __restrict__ out) {
+  __shared__ int leaf_lo[FM_MAX_LEAVES], leaf_n[FM_MAX_LEAVES];
+  __shared__ double leaf_sum[FM_MAX_LEAVES];
+  __shared__ int nleaves;
+  const int t = threadIdx.x;
+  const int good = status ? status[0] : 1;
+  int n = status ? status[1] : n_in;
+  n = n < 0 ? 0 : (n > FM_MAX_N ? FM_MAX_N : n);
+  if (t == 0) { nleaves = 0; pw_leaves(0, n, leaf_lo, leaf_n, &nleaves); }
+  __syncthreads();
+  for (int l = t; l < nleaves; l += FM_THREADS) leaf_sum[l] = pw_leaf(kp_ref, kp_cur, leaf_lo[l], leaf_n[l]);
+  __syncthreads();
+  if (t == 0) {
+    int next = 0;
+    const double sum = pw_combine(n, leaf_sum, &next);
+    out[0] = (double)good;
+    out[1] = (double)n;
+    out[2] = n > 0 ? sum / (double)n : 0.0;
+  }
+}
+
+int flow_mean(const double* kp_ref, const double* kp_cur, int n, const int32_t* status, double* out, cudaStream_t s) {
+  DFVO_REQUIRE(status != nullptr || (n >= 0 && n <= FM_MAX_N), DFVO_EINVAL, "flow_mean: n=%d (max %d)", n, FM_MAX_N);
+  DFVO_LAUNCH(k_flow_mean, dim3(1), dim3(FM_THREADS), 0, s, kp_ref, kp_cur, n, status, out);
+  DFVO_CHECK_LAUNCH();
+  return DFVO_OK;
+}
+
 int gather_keypoints(const int32_t* idx, const int32_t* cell_counts, int ncells, int n_best, const float* flow, int H, int W,
                      double* kp1, double* kp2, int32_t* n_out, cudaStream_t s) {
   DFVO_REQUIRE(ncells > 0 && ncells <= 8192, DFVO_EINVAL, "gather_keypoints: ncells");

@@ -1,6 +1,6 @@
 """``EssTracker`` with the reference's interface (libs/tracker/E_tracker.py:129-705) on the dfvo_b200
-kernels: five repeated essential-matrix RANSACs (replaying OpenCV's sampling sequence), GRIC model
-selection, pose recovery, and scale recovery from triangulated-vs-CNN depth."""
+kernels: five repeated essential-matrix RANSACs (replaying OpenCV's sampling sequence), GRIC or flow-magnitude
+model selection, pose recovery, and scale recovery from triangulated-vs-CNN depth."""
 import copy
 
 import numpy as np
@@ -24,7 +24,7 @@ class EssTracker:
         self.prev_pose = SE3()
         self.cam_intrinsics = cam_intrinsics
         self.timers = timers
-        assert cfg.e_tracker.validity.method == "GRIC", "dfvo_b200 implements e_tracker.validity.method GRIC (the default)"
+        assert cfg.e_tracker.validity.method in ("GRIC", "flow"), "dfvo_b200 implements e_tracker.validity.method GRIC and flow"
         self.K = [float(cam_intrinsics.cx), float(cam_intrinsics.cy), float(cam_intrinsics.fx), float(cam_intrinsics.fy)]
 
     def compute_pose_2d2d(self, kp_ref, kp_cur, is_iterative):
@@ -32,7 +32,8 @@ class EssTracker:
         repeat = self.cfg.e_tracker.ransac.repeat if is_iterative else 3                 # :179
         r = tracking.compute_pose_2d2d(tracking.default_engine(), np.ascontiguousarray(kp_ref, np.float64),
                                        np.ascontiguousarray(kp_cur, np.float64), self.K, repeat=repeat,
-                                       reproj_thre=self.cfg.e_tracker.ransac.reproj_thre)
+                                       reproj_thre=self.cfg.e_tracker.ransac.reproj_thre, validity=self.cfg.e_tracker.validity.method,
+                                       flow_thre=self.cfg.e_tracker.validity.get("thre"))
         pose = SE3()
         pose.R = r["R"]
         pose.t = r["t"]

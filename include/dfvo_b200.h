@@ -230,6 +230,36 @@ int dfvo_essential_tail(const double* E, const int32_t* info, const double* gric
                         double fx, double fy, double cx, double cy, const double* h_gric, const float* depth, int H, int W,
                         int min_samples, int max_trials, double stop_prob, double threshold, void* workspace, size_t workspace_bytes,
                         double* res, uint8_t* pose_mask, int32_t* pose_info, void* stream);
+/* dfvo_essential_tail for e_tracker.validity.method 'flow' (E_tracker.py:182-186,249-257,289-300), called only when the flow gate
+ * (dfvo_flow_mean > thre) passed -- a closed gate draws no shuffle and runs no essential matrix.  In one enqueue: every repeat's
+ * cv2.recoverPose(E_r, kp_cur[perm_r], kp_ref[perm_r]) count cnt_r (one launch; a count, so independent of the permutation), the
+ * best repeat = the first with inliers_r > best AND cnt_r > 0.05 N, the vote sum(cnt_r > 0.1 N) > R / 2, recoverPose on the best E,
+ * the cheirality gate and -- when depth != NULL -- the scale recovery of dfvo_essential_tail.  Arguments and res as
+ * dfvo_essential_tail's, except: no homography, res[319] = 0 and res[335..335+R) = cnt_r.  With depth == NULL res[0..316] are
+ * left as they were (no generator draw).  N <= 4096, R <= 32. */
+size_t dfvo_essential_flow_tail_workspace_bytes(int N, int R);
+int dfvo_essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx,
+                             double fy, double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials,
+                             double stop_prob, double threshold, void* workspace, size_t workspace_bytes, double* res, uint8_t* pose_mask,
+                             int32_t* pose_info, void* stream);
+/* The flow-magnitude gate of the E-tracker (E_tracker.py:182-185): np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1)), bit-equal to
+ * NumPy (rounded products and sums, NumPy's pairwise summation order).  kp [n][2] float64 (device).  status: NULL, or the device
+ * status of dfvo_local_bestn ({good, n, ...}), which then supplies the count -- so the selection's one status read also carries
+ * the mean.  out (device, 3 doubles) = {good (1 without status), n, mean}.  n <= 65536. */
+int dfvo_flow_mean(const double* kp_ref, const double* kp_cur, int n, const int32_t* status, double* out, void* stream);
+/* First half of the fused PnP tracker (pnp_tracker.py:45-94): keep the pairs whose kp_cur lies inside the H x W image, read the
+ * reference depth [H][W] float32 at int(kp_ref), keep 0 != d, min_depth < d < max_depth, compact in order and unproject:
+ * obj [m][3] = (inv(K) [u v 1]^T) d with NumPy's rounding, img [m][2] = kp_cur.  iK_host: inv(K) as np.linalg.inv gives it, row-major
+ * [9] in HOST memory (its off-diagonal zeros are checked).  count (device, 1 int32) = m. */
+int dfvo_pnp_filter(const double* kp_ref, const double* kp_cur, int n, const float* depth, int H, int W, double min_depth,
+                    double max_depth, const double* iK_host, double* obj, double* img, int32_t* count, void* stream);
+/* Second half: dfvo_pnp_ransac on the filtered points (N = m >= 5, perm = the host's R shuffles of arange(m), subsets =
+ * dfvo_cv_subset_stream_host(m, 5, iters)) and the best repeat (found && inliers > best, first maximum; pnp_tracker.py:108-110).
+ * res (device, 8 + 4 R doubles) = {best (-1: none), inliers, rvec[3], tvec[3], info [R][4]}. */
+size_t dfvo_pnp_tail_workspace_bytes(int N, int R, int iters);
+int dfvo_pnp_tail(const double* obj, const double* img, int N, const int32_t* perm, int R, const int32_t* subsets, int iters,
+                  double fx, double fy, double cx, double cy, double threshold, double prob, void* workspace,
+                  size_t workspace_bytes, double* res, void* stream);
 /* cv::triangulatePoints([I|0], T_21[:3], x1, x2) followed by X2 = T_21[:3] X / X_w (ops_3d.py:44-67): x1, x2
  * [N][2] normalised (float64), T21 [12] row-major 3x4 -> depth2 [N] = z of the point in view 2. */
 int dfvo_triangulate_depth(const double* x1, const double* x2, int N, const double* T21, double* depth2, void* stream);
