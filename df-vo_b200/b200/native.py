@@ -19,6 +19,24 @@ PREC_NAMES = {"fp32": PREC_FP32, "bf16": PREC_BF16, "tf32": PREC_TF32}
 NET_LITEFLOWNET, NET_MONODEPTH2 = 0, 1
 ACT_NONE, ACT_LEAKY, ACT_RELU, ACT_ELU, ACT_SIGMOID = 0, 1, 2, 3, 4
 
+# offsets (in doubles) of the packed results of dfvo_essential_tail / dfvo_scale_ransac and dfvo_pnp_tail (the DFVO_TAIL_* and
+# DFVO_PNP_* enums of include/dfvo_b200.h)
+DFVO_TAIL_SCALE, DFVO_TAIL_STATUS, DFVO_TAIL_TRIALS, DFVO_TAIL_INLIERS = 0, 1, 2, 3
+DFVO_TAIL_MT, DFVO_TAIL_MT_DOUBLES, DFVO_TAIL_SCALE_IO = 4, 313, 317
+DFVO_TAIL_BEST, DFVO_TAIL_VALID, DFVO_TAIL_HGRIC, DFVO_TAIL_CHEIR, DFVO_TAIL_NVALID, DFVO_TAIL_GATE = 317, 318, 319, 320, 321, 322
+DFVO_TAIL_RT, DFVO_TAIL_EGRIC = 323, 335
+DFVO_PNP_BEST, DFVO_PNP_INLIERS, DFVO_PNP_RVEC, DFVO_PNP_TVEC, DFVO_PNP_INFO = 0, 1, 2, 5, 8
+
+
+def tail_result_doubles(R):
+    """Length of dfvo_essential_tail's res for R repeats."""
+    return DFVO_TAIL_EGRIC + 5 * R
+
+
+def pnp_result_doubles(R):
+    """Length of dfvo_pnp_tail's res for R repeats."""
+    return DFVO_PNP_INFO + 4 * R
+
 c_int, c_void_p, c_char_p, c_float, c_double = (ctypes.c_int, ctypes.c_void_p, ctypes.c_char_p,
                                                ctypes.c_float, ctypes.c_double)
 c_size_t = ctypes.c_size_t
@@ -82,10 +100,6 @@ SIGNATURES = {
     "dfvo_essential_tail": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double,
                                     c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p,
                                     c_void_p, c_void_p]),
-    "dfvo_essential_flow_tail_workspace_bytes": (c_size_t, [c_int, c_int]),
-    "dfvo_essential_flow_tail": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double,
-                                         c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p,
-                                         c_void_p, c_void_p]),
     "dfvo_flow_mean": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "dfvo_pnp_filter": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_void_p, c_void_p,
                                 c_void_p, c_void_p]),

@@ -245,9 +245,7 @@ class FramePipeline:
             return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
         iterative = c.scale_recovery.method == "iterative"
         if not iterative and 10 < n <= eng.TAIL_MAX_N and self.fused_tail:
-            if self.validity == "flow":
-                return self.track_fused_flow_launch(cur, ref, kp1_buf, kp2_buf, n, flow_mean)
-            return self.track_fused_launch(cur, ref, kp1_buf, kp2_buf, n)
+            return self.track_fused_launch(cur, ref, kp1_buf, kp2_buf, n, flow_mean)
         return dict(pose=self.track_stepwise(cur, ref, kp1_buf, kp2_buf, n))
 
     def track_finish(self, tok):
@@ -272,7 +270,6 @@ class FramePipeline:
                                        kp_ref_buf=kp1_buf, kp_cur_buf=kp2_buf, defer_validity=True, validity=self.validity,
                                        flow_thre=c.e_tracker.validity.get("thre"))
         prep = None
-        iterative = c.scale_recovery.method == "iterative"
         if np.linalg.norm(r["t"]) != 0 and not iterative:
             E_spec = np.eye(4)
             E_spec[:3, :3], E_spec[:3, 3:] = r["R"], r["t"]
@@ -295,43 +292,26 @@ class FramePipeline:
             self.last["mode"] = "PnP"
         return hybrid
 
-    def track_fused_launch(self, cur, ref, kp1_buf, kp2_buf, n):
+    def track_fused_launch(self, cur, ref, kp1_buf, kp2_buf, n, flow_mean=None):
         """The E branch of `track` with the device-side tail (tracking.Engine.essential_tail): after the keypoint count is known the
         host draws the five shuffles, enqueues the homography model, the essential-matrix repeats and the fused tail, and reads ONE
         packed result -- instead of eleven small reads with host arithmetic in between (keypoints, RANSAC info, GRIC, mask, pose,
         cheirality, triangulated depths, CNN depths, H-GRIC, scale).  Same decisions, same generator stream; the host copies of the
-        keypoints are fetched only when the PnP fallback needs them."""
+        keypoints are fetched only when the PnP fallback needs them.
+        flow_mean (e_tracker.validity.method 'flow', E_tracker.py:182-186,249-257): the mean flow magnitude the selection read
+        returned.  A closed gate draws no shuffle and leaves E_pose at identity, so the PnP fallback runs; otherwise the tail uses
+        the flow-mode validity and no homography is launched."""
         c, eng, K = self.cfg, self.eng, self.K
+        if flow_mean is not None:
+            self.last["flow_mean"] = flow_mean
+            if not flow_mean > c.e_tracker.validity.thre:
+                self.last.update(valid=False, inliers=np.ones(n, bool), mode="PnP", scale=None)
+                return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
         rs = c.scale_recovery.ransac
-        perms = []
-        for _ in range(c.e_tracker.ransac.repeat):
-            order = np.arange(0, n, 1)
-            self.rng.shuffle(order)
-            perms.append(order)
-        h = eng.homography_launch(kp2_buf, kp1_buf, n)
+        perms = tracking.shuffles(self.rng, n, c.e_tracker.ransac.repeat)
+        h = eng.homography_launch(kp2_buf, kp1_buf, n) if flow_mean is None else None
         w = eng.essential_launch(kp2_buf, kp1_buf, n, perms, K, threshold=c.e_tracker.ransac.reproj_thre)
         tail = eng.essential_tail_launch(w, h, kp2_buf, kp1_buf, n, K, cur.depth, self.rng, rs.min_samples, rs.max_trials, rs.stop_prob, rs.thre)
-        return dict(tail=tail, w=w, ref=ref, kp1_buf=kp1_buf, kp2_buf=kp2_buf, n=n, last=self.last)
-
-    def track_fused_flow_launch(self, cur, ref, kp1_buf, kp2_buf, n, flow_mean):
-        """track_fused_launch for e_tracker.validity.method 'flow' (E_tracker.py:182-186,249-257): the gate on the mean flow magnitude
-        the selection read returned; a closed gate draws no shuffle and leaves E_pose at identity, so the PnP fallback runs.  Otherwise
-        the shuffles, the essential-matrix repeats and the flow-mode tail (Engine.essential_flow_tail_launch), read once by
-        track_fused_finish."""
-        c, eng, K = self.cfg, self.eng, self.K
-        self.last["flow_mean"] = flow_mean
-        if not flow_mean > c.e_tracker.validity.thre:
-            self.last.update(valid=False, inliers=np.ones(n, bool), mode="PnP", scale=None)
-            return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
-        rs = c.scale_recovery.ransac
-        perms = []
-        for _ in range(c.e_tracker.ransac.repeat):
-            order = np.arange(0, n, 1)
-            self.rng.shuffle(order)
-            perms.append(order)
-        w = eng.essential_launch(kp2_buf, kp1_buf, n, perms, K, threshold=c.e_tracker.ransac.reproj_thre)
-        tail = eng.essential_flow_tail_launch(w, kp2_buf, kp1_buf, n, K, cur.depth, self.rng, rs.min_samples, rs.max_trials, rs.stop_prob,
-                                              rs.thre)
         return dict(tail=tail, w=w, ref=ref, kp1_buf=kp1_buf, kp2_buf=kp2_buf, n=n, last=self.last)
 
     def pnp_fused_launch(self, kp1_buf, kp2_buf, n, ref=None):

@@ -21,6 +21,34 @@ def depth_constants(dataset):
     return TUM_DEPTH if "tum" in dataset else KITTI_DEPTH
 
 
+def shuffles(rng, n, repeat):
+    """The reference's per-repeat shuffles (E_tracker.py:225-226, pnp_tracker.py:90-95): `repeat` permutations of arange(n), each
+    drawn by rng.shuffle in turn, so the generator advances exactly as in the reference."""
+    perms = []
+    for _ in range(repeat):
+        order = np.arange(0, n, 1)
+        rng.shuffle(order)
+        perms.append(order)
+    return perms
+
+
+def _mt_state_in(rng, block, who):
+    """Write `rng`'s MT19937 state into the result block (host float64 array) at DFVO_TAIL_MT; returns the state."""
+    st = rng.get_state()
+    if st[0] != "MT19937":
+        raise TypeError("%s needs a legacy MT19937 generator (np.random / np.random.RandomState)" % who)
+    u = block[native.DFVO_TAIL_MT:native.DFVO_TAIL_SCALE_IO].view(np.uint32)
+    u[:624] = st[1]
+    u[624] = st[2]
+    return st
+
+
+def _mt_state_out(rng, block, st):
+    """Install the advanced MT19937 state the device left in the result block into `rng` (`st`: the state written at launch)."""
+    u = block[native.DFVO_TAIL_MT:native.DFVO_TAIL_SCALE_IO].view(np.uint32)
+    rng.set_state(("MT19937", u[:624].copy(), int(u[624]), st[3], st[4]))
+
+
 class Engine:
     """One ``dfvo_ctx`` + its buffers for a fixed image size."""
 
@@ -258,11 +286,14 @@ class Engine:
 
     def essential_tail(self, w, h, kp_cur_buf, kp_ref_buf, n, K, depth_buf, rng, min_samples=3, max_trials=100, stop_prob=0.99, thre=0.1):
         """Everything between the essential-matrix repeats and "pose and scale known" in one enqueue and ONE device->host read
-        (dfvo_essential_tail): best repeat, recoverPose, the GRIC vote against the homography handle `h`, the cheirality gate, the depth
-        ratios and the scale regressor (with `rng`'s MT19937 state; the advanced state is installed back).  Returns a dict with
-        R, t (identity / zero when the pose is rejected, as compute_pose_2d2d + resolve_validity give them), valid, cheirality, best,
-        E_gric, H_gric, ransac_info, scale (-1 when not recovered), scale_status, and `w` for a lazy inlier mask.
-        = essential_tail_launch + essential_tail_finish; between the two `rng` must not be used (its state travels with the launch)."""
+        (dfvo_essential_tail): best repeat, recoverPose, the validity vote, the cheirality gate, the depth ratios and the scale
+        regressor (with `rng`'s MT19937 state; the advanced state is installed back).  `h`: the homography handle for GRIC validity,
+        or None for e_tracker.validity.method 'flow' (the caller took the flow gate before drawing the shuffles of `w`).
+        `depth_buf` None: pose only (no scale recovery, `rng` untouched).  Returns a dict with R, t (identity / zero when the pose is
+        rejected, as compute_pose_2d2d + resolve_validity give them), valid, cheirality, best, E_gric (flow: the per-repeat
+        cheirality counts), H_gric (flow: 0), ransac_info, scale (-1 when not recovered), scale_status, and `w` for a lazy inlier
+        mask.  = essential_tail_launch + essential_tail_finish; between the two `rng` must not be used (its state travels with the
+        launch)."""
         return self.essential_tail_finish(self.essential_tail_launch(w, h, kp_cur_buf, kp_ref_buf, n, K, depth_buf, rng, min_samples,
                                                                      max_trials, stop_prob, thre))
 
@@ -273,66 +304,37 @@ class Engine:
         c = getattr(self, "_tail", None)
         if c is None or c["cap"] < cap or c["R"] != R:
             nb = int(self.lib.dfvo_essential_tail_workspace_bytes(cap))
-            c = self._tail = dict(cap=cap, R=R, ws=self.rt.empty((nb,), np.uint8), res=self.rt.empty((335 + 5 * R,), np.float64),
-                                  host=np.zeros(335 + 5 * R, np.float64))
-        st = rng.get_state()
-        if st[0] != "MT19937":
-            raise TypeError("essential_tail needs a legacy MT19937 generator (np.random / np.random.RandomState)")
-        u = c["host"][4:317].view(np.uint32)
-        u[:624] = st[1]
-        u[624] = st[2]
+            size = native.tail_result_doubles(R)
+            c = self._tail = dict(cap=cap, R=R, ws=self.rt.empty((nb,), np.uint8), res=self.rt.empty((size,), np.float64),
+                                  host=np.zeros(size, np.float64))
+        st = _mt_state_in(rng, c["host"], "essential_tail")
         c["res"].upload(c["host"])
-        self.rt.wait_event(h["done"])                               # order this stream after the homography side stream
-        self.lib.check(self.lib.dfvo_essential_tail(w["E"].ptr, w["info"].ptr, w["gric"].ptr, R, kp_cur_buf.ptr, kp_ref_buf.ptr, n, fx, fy,
-                                                    cx, cy, h["gric"].ptr, depth_buf.ptr, self.H, self.W, int(min_samples), int(max_trials),
-                                                    float(stop_prob), float(thre), c["ws"].ptr, c["ws"].shape[0], c["res"].ptr,
-                                                    w["pmask"].ptr, w["pinfo"].ptr, self.rt.stream_ptr()))
+        gric = h_gric = None                                        # flow validity: no homography
+        if h is not None:
+            self.rt.wait_event(h["done"])                           # order this stream after the homography side stream
+            gric, h_gric = w["gric"].ptr, h["gric"].ptr
+        self.lib.check(self.lib.dfvo_essential_tail(w["E"].ptr, w["info"].ptr, gric, R, kp_cur_buf.ptr, kp_ref_buf.ptr, n, fx, fy, cx, cy,
+                                                    h_gric, depth_buf.ptr if depth_buf is not None else None, self.H, self.W,
+                                                    int(min_samples), int(max_trials), float(stop_prob), float(thre), c["ws"].ptr,
+                                                    c["ws"].shape[0], c["res"].ptr, w["pmask"].ptr, w["pinfo"].ptr, self.rt.stream_ptr()))
         return dict(c=c, w=w, n=n, R=R, rng=rng, st=st)
 
     def essential_tail_finish(self, tok):
         c, w, n, R, rng, st = tok["c"], tok["w"], tok["n"], tok["R"], tok["rng"], tok["st"]
         o = c["res"].numpy()                                        # the one synchronising read
-        u = o[4:317].view(np.uint32)
-        rng.set_state(("MT19937", u[:624].copy(), int(u[624]), st[3], st[4]))
-        best, valid, cheir = int(o[317]), bool(o[318]), int(o[320])
-        out = dict(R=np.eye(3), t=np.zeros((3, 1)), valid=valid, cheirality=0, best=best, H_gric=float(o[319]),
-                   E_gric=o[335:335 + R].copy(), ransac_info=o[335 + R:335 + 5 * R].reshape(R, 4).astype(np.int32), scale=-1,
-                   scale_status=int(o[1]), n_ratios=int(o[321]), handle=w)
+        _mt_state_out(rng, o, st)
+        best, valid, cheir = int(o[native.DFVO_TAIL_BEST]), bool(o[native.DFVO_TAIL_VALID]), int(o[native.DFVO_TAIL_CHEIR])
+        status, e0, rt0 = o[native.DFVO_TAIL_STATUS], native.DFVO_TAIL_EGRIC, native.DFVO_TAIL_RT
+        out = dict(R=np.eye(3), t=np.zeros((3, 1)), valid=valid, cheirality=0, best=best, H_gric=float(o[native.DFVO_TAIL_HGRIC]),
+                   E_gric=o[e0:e0 + R].copy(), ransac_info=o[e0 + R:e0 + 5 * R].reshape(R, 4).astype(np.int32), scale=-1,
+                   scale_status=int(status), n_ratios=int(o[native.DFVO_TAIL_NVALID]), handle=w)
         if valid and best >= 0 and cheir > n * 0.1:
-            out["R"], out["t"], out["cheirality"] = o[323:332].reshape(3, 3).copy(), o[332:335].reshape(3, 1).copy(), cheir
-        if o[1] == -1:
+            out["R"], out["t"], out["cheirality"] = o[rt0:rt0 + 9].reshape(3, 3).copy(), o[rt0 + 9:rt0 + 12].reshape(3, 1).copy(), cheir
+        if status == -1:
             raise ValueError("RANSAC could not find a valid consensus set")
-        if o[1] == 1:
-            out["scale"] = float(o[0])
+        if status == 1:
+            out["scale"] = float(o[native.DFVO_TAIL_SCALE])
         return out
-
-    def essential_flow_tail_launch(self, w, kp_cur_buf, kp_ref_buf, n, K, depth_buf, rng, min_samples=3, max_trials=100, stop_prob=0.99,
-                                   thre=0.1):
-        """:meth:`essential_tail_launch` for e_tracker.validity.method 'flow' (dfvo_essential_flow_tail): the per-repeat recoverPose
-        counts, the flow-mode best-E rule and vote, then the same recoverPose / cheirality gate / scale recovery.  The caller took the
-        flow gate before drawing the shuffles of `w`.  depth_buf None: pose only (no scale recovery, `rng` untouched).  Finish with
-        :meth:`essential_tail_finish`; its E_gric holds the per-repeat cheirality counts, H_gric is 0."""
-        cx, cy, fx, fy = K
-        R = w["info"].shape[0]
-        cap = w["cap"]
-        c = getattr(self, "_ftail", None)
-        if c is None or c["cap"] < cap or c["R"] != R:
-            nb = int(self.lib.dfvo_essential_flow_tail_workspace_bytes(cap, R))
-            c = self._ftail = dict(cap=cap, R=R, ws=self.rt.empty((nb,), np.uint8), res=self.rt.empty((335 + 5 * R,), np.float64),
-                                   host=np.zeros(335 + 5 * R, np.float64))
-        st = rng.get_state()
-        if st[0] != "MT19937":
-            raise TypeError("essential_flow_tail needs a legacy MT19937 generator (np.random / np.random.RandomState)")
-        u = c["host"][4:317].view(np.uint32)
-        u[:624] = st[1]
-        u[624] = st[2]
-        c["res"].upload(c["host"])
-        self.lib.check(self.lib.dfvo_essential_flow_tail(w["E"].ptr, w["info"].ptr, R, kp_cur_buf.ptr, kp_ref_buf.ptr, n, fx, fy, cx, cy,
-                                                         depth_buf.ptr if depth_buf is not None else None, self.H, self.W,
-                                                         int(min_samples), int(max_trials), float(stop_prob), float(thre), c["ws"].ptr,
-                                                         c["ws"].shape[0], c["res"].ptr, w["pmask"].ptr, w["pinfo"].ptr,
-                                                         self.rt.stream_ptr()))
-        return dict(c=c, w=w, n=n, R=R, rng=rng, st=st)
 
     def pnp_tail_launch(self, kp_ref_buf, kp_cur_buf, n, depth_buf, K, min_depth, max_depth, rng, repeat=5, iters=100, reproj_thre=1.0,
                         prob=0.99):
@@ -351,11 +353,7 @@ class Engine:
                                                 float(max_depth), iK.ctypes.data_as(ctypes.c_void_p), f["obj"].ptr, f["img"].ptr,
                                                 f["m"].ptr, self.rt.stream_ptr()))
         m = int(f["m"].numpy()[0])                                        # the one read before the solver
-        perms = []
-        for _ in range(repeat):                                           # pnp_tracker.py:90-95
-            order = np.arange(0, m, 1)
-            rng.shuffle(order)
-            perms.append(order)
+        perms = shuffles(rng, m, repeat)                                  # pnp_tracker.py:90-95
         if m <= 4:                                                        # pnp_tracker.py:97: no solver, identity
             return dict(m=m, res=None)
         key = (repeat, iters)
@@ -364,7 +362,7 @@ class Engine:
             cap = self._capacity(m)
             nb = int(self.lib.dfvo_pnp_tail_workspace_bytes(cap, repeat, iters))
             c = self._pnp_ws[("tail",) + key] = dict(cap=cap, ws=self.rt.empty((nb,), np.uint8), perm_c=self.rt.empty((repeat * cap,), np.int32),
-                                                     res=self.rt.empty((8 + 4 * repeat,), np.float64))
+                                                     res=self.rt.empty((native.pnp_result_doubles(repeat),), np.float64))
         perm = c["perm_c"].view((repeat, m)).upload(np.asarray(perms, np.int32))
         self.lib.check(self.lib.dfvo_pnp_tail(f["obj"].ptr, f["img"].ptr, m, perm.ptr, repeat, self._subset_table(m, iters).ptr, iters,
                                               fx, fy, cx, cy, float(reproj_thre), prob, c["ws"].ptr, c["ws"].shape[0], c["res"].ptr,
@@ -378,10 +376,10 @@ class Engine:
         best_inl = 0
         if tok["res"] is not None:
             o = tok["res"].numpy()                                        # the one packed read
-            if o[0] >= 0:
-                best_inl = int(o[1])
-                pose[:3, :3] = hostmath.rodrigues(o[2:5].copy())
-                pose[:3, 3] = o[5:8]
+            if o[native.DFVO_PNP_BEST] >= 0:
+                best_inl = int(o[native.DFVO_PNP_INLIERS])
+                pose[:3, :3] = hostmath.rodrigues(o[native.DFVO_PNP_RVEC:native.DFVO_PNP_RVEC + 3].copy())
+                pose[:3, 3] = o[native.DFVO_PNP_TVEC:native.DFVO_PNP_TVEC + 3]
         return np.linalg.inv(pose), best_inl, tok["m"]
 
     def recover_pose(self, w, best, kp_cur_buf, kp_ref_buf, n, K):
@@ -448,27 +446,22 @@ class Engine:
         consensus set exists."""
         ratio = np.ascontiguousarray(ratio, np.float64).reshape(-1)
         n = ratio.shape[0]
-        st = rng.get_state()
-        if st[0] != "MT19937":
-            raise TypeError("ransac_scale needs a legacy MT19937 generator (np.random / np.random.RandomState)")
+        io_h = np.zeros(native.DFVO_TAIL_SCALE_IO, np.float64)
+        st = _mt_state_in(rng, io_h, "ransac_scale")
         cap = self._capacity(n)
         if not hasattr(self, "_sr") or self._sr["x"].size < cap:
-            self._sr = dict(x=self.rt.empty((cap,), np.float64), io=self.rt.empty((4 + 313,), np.float64), perm=self.rt.empty((cap,), np.int32))
+            self._sr = dict(x=self.rt.empty((cap,), np.float64), io=self.rt.empty((native.DFVO_TAIL_SCALE_IO,), np.float64),
+                            perm=self.rt.empty((cap,), np.int32))
         w = self._sr
         w["x"].view((n,)).upload(ratio)
-        io_h = np.zeros(4 + 313, np.float64)
-        u = io_h[4:].view(np.uint32)
-        u[:624] = st[1]
-        u[624] = st[2]
         w["io"].upload(io_h)
         self.lib.check(self.lib.dfvo_scale_ransac(w["x"].ptr, n, int(min_samples), int(max_trials), float(stop_prob), float(thre), w["io"].ptr,
                                                   w["perm"].ptr, self.rt.stream_ptr()))
         out = w["io"].numpy()
-        u = out[4:].view(np.uint32)
-        rng.set_state(("MT19937", u[:624].copy(), int(u[624]), st[3], st[4]))
-        if out[1] < 0:
+        _mt_state_out(rng, out, st)
+        if out[native.DFVO_TAIL_STATUS] < 0:
             raise ValueError("RANSAC could not find a valid consensus set")
-        return float(out[0])
+        return float(out[native.DFVO_TAIL_SCALE])
 
     def triangulate_depth(self, kp1n_buf, kp2n_buf, n, T21):
         if not hasattr(self, "_tri") or self._tri["z"].shape[0] < n:
@@ -480,36 +473,46 @@ class Engine:
 
 
 # ---------------------------------------------------------------------------------------------
-# host-level orchestration of the E-tracker (E_tracker.py:154-307, validity.method == 'GRIC')
+# host-level orchestration of the E-tracker (E_tracker.py:154-307)
 # ---------------------------------------------------------------------------------------------
 def compute_pose_2d2d(engine, kp_ref, kp_cur, K, repeat=5, reproj_thre=0.2, rng=np.random, kp_ref_buf=None, kp_cur_buf=None,
                       defer_validity=False, validity="GRIC", flow_thre=None):
-    """Same contract as ``EssTracker.compute_pose_2d2d`` with the default GRIC validity check (validity='flow': the flow-magnitude
-    check with threshold `flow_thre`, see :func:`_compute_pose_2d2d_flow`).
+    """Same contract as ``EssTracker.compute_pose_2d2d`` with the GRIC validity check, or (validity='flow') the flow-magnitude
+    check with threshold `flow_thre`.
     kp_ref/kp_cur: float64 [N,2] host arrays (device copies optional).  Everything numeric runs on the device: the
     homography model + GRIC-H (csrc/homog.cu), the five essential-matrix RANSAC repeats + GRIC-E (ransac.cu) and
     recoverPose; the host draws the shuffles, takes the majority vote and the cheirality decision.
     Returns dict(R, t, inliers, valid, cheirality).
 
-    defer_validity=True: R, t are the pose *as if* the E-model is valid and the caller must call
+    GRIC, defer_validity=True: R, t are the pose *as if* the E-model is valid and the caller must call
     :func:`resolve_validity` (which resets them to identity / zero when GRIC prefers the homography) before using them
-    for a decision; lets a caller issue pose-dependent device work before it reads the vote.  Results are identical."""
+    for a decision; lets a caller issue pose-dependent device work before it reads the vote.  Results are identical.
+
+    flow (E_tracker.py:182-186,249-257,289-300): the gate mean |kp_ref - kp_cur| > thre is NumPy's own expression on the host
+    arrays; a closed gate draws no shuffle and leaves the pose at identity.  Otherwise the repeats, the per-repeat recoverPose
+    counts, the flow-mode best-E rule, the vote and the final recoverPose run on the device (essential_ransac + the essential tail
+    without scale recovery) and are read once."""
     n = kp_ref.shape[0]
     R, t = np.eye(3), np.zeros((3, 1))
     out = dict(R=R, t=t, inliers=np.ones(n, bool), valid=False, cheirality=0)
     if validity == "flow":
-        return _compute_pose_2d2d_flow(engine, kp_ref, kp_cur, K, repeat, reproj_thre, rng, kp_ref_buf, kp_cur_buf, flow_thre, out)
-    if n <= 10:                                                     # E_tracker.py:196,216-217
+        out["flow_mean"] = np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1))
+        if not out["flow_mean"] > flow_thre:
+            return out
+    elif n <= 10:                                                   # E_tracker.py:196,216-217
         return out
-    # host RNG consumption identical to the reference: one shuffle per repeat (E_tracker.py:225-226)
-    perms = []
-    for _ in range(repeat):
-        order = np.arange(0, n, 1)
-        rng.shuffle(order)
-        perms.append(order)
+    perms = shuffles(rng, n, repeat)                                # host RNG consumption identical to the reference
     rt = engine.rt
     kp_cur_buf = kp_cur_buf or rt.from_host(kp_cur)
     kp_ref_buf = kp_ref_buf or rt.from_host(kp_ref)
+    if validity == "flow":
+        w = engine.essential_launch(kp_cur_buf, kp_ref_buf, n, perms, K, threshold=reproj_thre)
+        o = engine.essential_tail(w, None, kp_cur_buf, kp_ref_buf, n, K, None, rng)
+        out.update(valid=o["valid"], cheirality=o["cheirality"], R=o["R"], t=o["t"], ransac_info=o["ransac_info"],
+                   cheirality_counts=o["E_gric"])
+        if o["best"] >= 0:
+            out["inliers"] = w["mask"].numpy()[o["best"]].astype(bool)
+        return out
     h = engine.homography_launch(kp_cur_buf, kp_ref_buf, n)         # homography model (E_tracker.py:199-215)
     w = engine.essential_launch(kp_cur_buf, kp_ref_buf, n, perms, K, threshold=reproj_thre)
     info = w["info"].numpy()
@@ -529,32 +532,6 @@ def compute_pose_2d2d(engine, kp_ref, kp_cur, K, repeat=5, reproj_thre=0.2, rng=
     out["_vote"] = (h, gric, repeat, best)
     if not defer_validity:
         resolve_validity(out)
-    return out
-
-
-def _compute_pose_2d2d_flow(engine, kp_ref, kp_cur, K, repeat, reproj_thre, rng, kp_ref_buf, kp_cur_buf, flow_thre, out):
-    """E_tracker.py:182-186,249-257,289-300 (validity.method 'flow'): the gate mean |kp_ref - kp_cur| > thre is NumPy's own expression
-    on the host arrays; a closed gate draws no shuffle and leaves the pose at identity.  Otherwise the repeats, the per-repeat
-    recoverPose counts, the flow-mode best-E rule, the vote and the final recoverPose run on the device (essential_ransac +
-    dfvo_essential_flow_tail without scale recovery) and are read once."""
-    n = kp_ref.shape[0]
-    avg_flow = np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1))
-    out["flow_mean"] = avg_flow
-    if not avg_flow > flow_thre:
-        return out
-    perms = []
-    for _ in range(repeat):
-        order = np.arange(0, n, 1)
-        rng.shuffle(order)
-        perms.append(order)
-    rt = engine.rt
-    kp_cur_buf = kp_cur_buf or rt.from_host(kp_cur)
-    kp_ref_buf = kp_ref_buf or rt.from_host(kp_ref)
-    w = engine.essential_launch(kp_cur_buf, kp_ref_buf, n, perms, K, threshold=reproj_thre)
-    o = engine.essential_tail_finish(engine.essential_flow_tail_launch(w, kp_cur_buf, kp_ref_buf, n, K, None, rng))
-    out.update(valid=o["valid"], cheirality=o["cheirality"], R=o["R"], t=o["t"], ransac_info=o["ransac_info"], cheirality_counts=o["E_gric"])
-    if o["best"] >= 0:
-        out["inliers"] = w["mask"].numpy()[o["best"]].astype(bool)
     return out
 
 
@@ -584,11 +561,7 @@ def compute_pose_3d2d(engine, kp1, kp2, d, K, repeat=5, iters=100, reproj_thre=1
     n = kp1.shape[0]
     Kmat = np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1.0]])
     XYZ = (np.linalg.inv(Kmat) @ np.concatenate([kp1, np.ones((n, 1))], 1).T).T * np.asarray(d, np.float64)[:, None]
-    perms = []
-    for _ in range(repeat):
-        order = np.arange(0, n, 1)
-        rng.shuffle(order)
-        perms.append(order)
+    perms = shuffles(rng, n, repeat)
     pose = np.eye(4)
     best_inl = 0
     if n > 4:                                                       # pnp_tracker.py:97

@@ -573,17 +573,6 @@ int dfvo_essential_tail(const double* E, const int32_t* info, const double* gric
   API_END
 }
 
-size_t dfvo_essential_flow_tail_workspace_bytes(int N, int R) { return essential_flow_tail_workspace_bytes(N, R); }
-int dfvo_essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx,
-                             double fy, double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials,
-                             double stop_prob, double threshold, void* workspace, size_t workspace_bytes, double* res, uint8_t* pose_mask,
-                             int32_t* pose_info, void* stream) {
-  API_BEGIN
-  return essential_flow_tail(E, info, R, kp_cur, kp_ref, N, fx, fy, cx, cy, depth, H, W, min_samples, max_trials, stop_prob, threshold,
-                             workspace, workspace_bytes, res, pose_mask, pose_info, (cudaStream_t)stream);
-  API_END
-}
-
 int dfvo_flow_mean(const double* kp_ref, const double* kp_cur, int n, const int32_t* status, double* out, void* stream) {
   API_BEGIN
   DFVO_REQUIRE(kp_ref && kp_cur && out, DFVO_EINVAL, "dfvo_flow_mean args");

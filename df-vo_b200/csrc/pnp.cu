@@ -847,10 +847,10 @@ __global__ void k_pnp_pick(const double* __restrict__ rt, const int32_t* __restr
   int best = -1, best_inl = 0;
   for (int r = 0; r < R; ++r)
     if (info[4 * r] && info[4 * r + 1] > best_inl) { best = r; best_inl = info[4 * r + 1]; }   // pnp_tracker.py:108-110
-  res[0] = (double)best;
-  res[1] = (double)best_inl;
-  for (int k = 0; k < 6; ++k) res[2 + k] = best >= 0 ? rt[6 * best + k] : 0.0;
-  for (int q = 0; q < 4 * R; ++q) res[8 + q] = (double)info[q];
+  res[DFVO_PNP_BEST] = (double)best;
+  res[DFVO_PNP_INLIERS] = (double)best_inl;
+  for (int k = 0; k < 6; ++k) res[DFVO_PNP_RVEC + k] = best >= 0 ? rt[6 * best + k] : 0.0;    // rvec, then tvec
+  for (int q = 0; q < 4 * R; ++q) res[DFVO_PNP_INFO + q] = (double)info[q];
 }
 
 size_t pnp_tail_workspace_bytes(int N, int R, int iters) { return pnp_workspace_bytes(N, R, iters) + (size_t)R * (6 * 8 + 4 * 4) + 256; }

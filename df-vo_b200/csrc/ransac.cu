@@ -566,9 +566,15 @@ k_scale_ransac(const double* __restrict__ x, int n, int min_samples, int max_tri
   // fused E-tracker tail: the sample count and the go / no-go decision live on the device (no generator draw when the gate is closed
   // or fewer than 11 depth ratios are valid, exactly where the reference does not call the regressor: E_tracker.py:617-643)
   if (gate != nullptr) {
-    if (*gate == 0.0) { if (threadIdx.x == 0) { io[0] = -1.0; io[1] = -3.0; io[2] = 0.0; io[3] = 0.0; } return; }
+    if (*gate == 0.0) {
+      if (threadIdx.x == 0) { io[DFVO_TAIL_SCALE] = -1.0; io[DFVO_TAIL_STATUS] = -3.0; io[DFVO_TAIL_TRIALS] = 0.0; io[DFVO_TAIL_INLIERS] = 0.0; }
+      return;
+    }
     n = (int)*n_dev;
-    if (n <= 10) { if (threadIdx.x == 0) { io[0] = -1.0; io[1] = -2.0; io[2] = 0.0; io[3] = 0.0; } return; }
+    if (n <= 10) {
+      if (threadIdx.x == 0) { io[DFVO_TAIL_SCALE] = -1.0; io[DFVO_TAIL_STATUS] = -2.0; io[DFVO_TAIL_TRIALS] = 0.0; io[DFVO_TAIL_INLIERS] = 0.0; }
+      return;
+    }
   }
   __shared__ uint32_t key[624];
   __shared__ int idx[SR_MAX_SAMPLES];
@@ -577,7 +583,7 @@ k_scale_ransac(const double* __restrict__ x, int n, int min_samples, int max_tri
   __shared__ double s_best_sh;
   __shared__ int go;
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  uint32_t* st = reinterpret_cast<uint32_t*>(io + 4);
+  uint32_t* st = reinterpret_cast<uint32_t*>(io + DFVO_TAIL_MT);
   for (int i = t; i < 624; i += SR_THREADS) key[i] = st[i];
   __syncthreads();
   Mt g; g.key = key; g.pos = (int)st[624];
@@ -667,10 +673,10 @@ k_scale_ransac(const double* __restrict__ x, int n, int min_samples, int max_tri
   if (t == 0) {
     double a = 0, b = 0; int c = 0;
     for (int w8 = 0; w8 < SR_THREADS / 32; ++w8) { a += part_d[0][w8]; b += part_d[1][w8]; c += part_i[w8]; }
-    io[0] = (have && b != 0.0) ? a / b : 0.0;
-    io[1] = have ? 1.0 : -1.0;
-    io[2] = (double)n_trials;
-    io[3] = (double)c;
+    io[DFVO_TAIL_SCALE] = (have && b != 0.0) ? a / b : 0.0;
+    io[DFVO_TAIL_STATUS] = have ? 1.0 : -1.0;
+    io[DFVO_TAIL_TRIALS] = (double)n_trials;
+    io[DFVO_TAIL_INLIERS] = (double)c;
     (void)s_best_sh;
   }
   __syncthreads();
@@ -689,53 +695,95 @@ int scale_ransac(const double* ratio, int n, int min_samples, int max_trials, do
 }
 
 // ------------------------------------------------------------------------------------------------
-// Fused tail of the E-tracker (E_tracker.py:270-300 + dfvo.py:165-193 + E_tracker.py:476-507,571-643): everything between "the five
-// RANSAC repeats are done" and "the host knows pose and scale" without a host round trip:
-//   k_track_pick   first repeat with the most inliers (E_tracker.py:278-281), its E, the per-repeat numbers as doubles
-//   recover_pose   cv2.recoverPose on that E (kernels above)
-//   k_track_gate   majority vote H_gric > E_gric (:286-290), cheirality > 0.1 n (:299-300), |t| != 0 (dfvo.py:182) -> gate; T_21 = inv([R|t])
-//   k_scale_chain  find_scale_from_depth up to the regressor: normalise, triangulate, CNN depth at int(kp_cur), last-writer-wins
-//                  per pixel, ratios in row-major pixel order (ops_3d.py:15-41, E_tracker.py:598-616)
-//   k_scale_ransac the regressor with the host generator's MT19937 state (above), gated
-// res (doubles): [0..3] scale io, [4..316] generator state, [317] best, [318] valid, [319] H_gric, [320] cheirality count, [321] valid
-// depth ratios, [322] gate, [323..334] Rt of recoverPose, [335..335+R) E_gric, then info [R][4].
+// Fused tail of the E-tracker (E_tracker.py:182-186,249-300 + dfvo.py:165-193 + E_tracker.py:476-507,571-643): everything between
+// "the five RANSAC repeats are done" and "the host knows pose and scale" without a host round trip.  The validity method decides the
+// pick: GRIC (h_gric != nullptr) or the flow magnitude (h_gric == nullptr; the caller took the gate mean flow > thre before it drew
+// the shuffles).
+//   k_recover_pose_counts  flow only: every repeat's recoverPose count (a count over all points, so the permutation drops out)
+//   k_track_pick           GRIC: first repeat with the most inliers (E_tracker.py:278-281), its E, the per-repeat numbers as doubles
+//   k_track_pick_flow      flow: first repeat with more inliers AND count > 0.05 n, the vote sum(count > 0.1 n) > R / 2
+//   recover_pose           cv2.recoverPose on the best E (kernels above)
+//   k_track_gate           GRIC: majority vote H_gric > E_gric (:286-290); cheirality > 0.1 n (:299-300), |t| != 0 (dfvo.py:182)
+//                          -> gate; T_21 = inv([R|t])
+//   k_scale_chain          find_scale_from_depth up to the regressor: normalise, triangulate, CNN depth at int(kp_cur),
+//                          last-writer-wins per pixel, ratios in row-major pixel order (ops_3d.py:15-41, E_tracker.py:598-616)
+//   k_scale_ransac         the regressor with the host generator's MT19937 state (above), gated
+// res layout: DFVO_TAIL_* (include/dfvo_b200.h).
 // ------------------------------------------------------------------------------------------------
-#define TR_BEST 317
-#define TR_VALID 318
-#define TR_HGRIC 319
-#define TR_CHEIR 320
-#define TR_NVALID 321
-#define TR_GATE 322
-#define TR_RT 323
-#define TR_EGRIC 335
+// every repeat's four candidate counts in one launch: grid (cdiv(4N, 256), R), counts [R][4] zeroed by the caller
+__global__ void __launch_bounds__(256)
+k_recover_pose_counts(const double* __restrict__ E, const double* __restrict__ p1, const double* __restrict__ p2, int N, double focal,
+                      double cx, double cy, double dist, int32_t* __restrict__ counts) {
+  __shared__ double sR[2][3][3], st[3];
+  __shared__ int cnt[4];
+  const int t = threadIdx.x, r = blockIdx.y;
+  if (t == 0) decompose_essential(E + 9 * r, sR, st);
+  if (t < 4) cnt[t] = 0;
+  __syncthreads();
+  const int g = blockIdx.x * 256 + t, j = g >> 2, k = g & 3;
+  const bool m = j < N && cheirality_ok(sR, st, k, p1, p2, j, focal, cx, cy, dist);
+  const unsigned ballot = __ballot_sync(0xffffffffu, m);
+  const int lane = t & 31;
+  if (lane < 4) {
+    const int c = __popc(ballot & (0x11111111u << lane));
+    if (c) atomicAdd(&cnt[lane], c);
+  }
+  __syncthreads();
+  if (t < 4 && cnt[t]) atomicAdd(&counts[4 * r + t], cnt[t]);
+}
+
+// what both pick rules store: the best repeat, info [R][4] as doubles, the best E (any finite E keeps the kernels benign when none)
+DFVO_D void track_pick_store(const int32_t* __restrict__ info, const double* __restrict__ E, int R, int best, double* __restrict__ res,
+                             double* __restrict__ E_best) {
+  res[DFVO_TAIL_BEST] = (double)best;
+  for (int q = 0; q < 4 * R; ++q) res[DFVO_TAIL_EGRIC + R + q] = (double)info[q];
+  for (int q = 0; q < 9; ++q) E_best[q] = best >= 0 ? E[9 * best + q] : ((q % 4 == 0 && q < 8) ? 1.0 : 0.0);
+}
 
 __global__ void k_track_pick(const int32_t* __restrict__ info, const double* __restrict__ gric, const double* __restrict__ E, int R,
                              double* __restrict__ res, double* __restrict__ E_best) {
   if (threadIdx.x != 0) return;
   int best = -1, cnt = 0;
-  for (int r = 0; r < R; ++r)
-    if (info[4 * r] > cnt) { best = r; cnt = info[4 * r]; }
-  res[TR_BEST] = (double)best;
   for (int r = 0; r < R; ++r) {
-    res[TR_EGRIC + r] = gric[r];
-    for (int q = 0; q < 4; ++q) res[TR_EGRIC + R + 4 * r + q] = (double)info[4 * r + q];
+    if (info[4 * r] > cnt) { best = r; cnt = info[4 * r]; }
+    res[DFVO_TAIL_EGRIC + r] = gric[r];
   }
-  for (int q = 0; q < 9; ++q) E_best[q] = best >= 0 ? E[9 * best + q] : ((q % 4 == 0 && q < 8) ? 1.0 : 0.0);    // any finite E keeps the kernels benign
+  track_pick_store(info, E, R, best, res, E_best);
 }
 
+__global__ void k_track_pick_flow(const int32_t* __restrict__ info, const int32_t* __restrict__ counts, const double* __restrict__ E, int R,
+                                  int n, double* __restrict__ res, double* __restrict__ E_best) {
+  if (threadIdx.x != 0) return;
+  int best = -1, best_inl = 0, votes = 0;
+  for (int r = 0; r < R; ++r) {
+    int b = 0;                                                         // recoverPose keeps the first candidate with the most points
+    for (int k = 1; k < 4; ++k) if (counts[4 * r + k] > counts[4 * r + b]) b = k;
+    const int c = counts[4 * r + b];
+    votes += ((double)c > (double)n * 0.1) ? 1 : 0;
+    if (info[4 * r] > best_inl && (double)c > (double)n * 0.05) { best = r; best_inl = info[4 * r]; }
+    res[DFVO_TAIL_EGRIC + r] = (double)c;
+  }
+  res[DFVO_TAIL_VALID] = ((double)votes > (double)R / 2.0) ? 1.0 : 0.0;
+  track_pick_store(info, E, R, best, res, E_best);
+}
+
+// h_gric == nullptr: the vote is the one k_track_pick_flow wrote
 __global__ void k_track_gate(double* __restrict__ res, const int32_t* __restrict__ pinfo, const double* __restrict__ h_gric, int R, int n,
                              double* __restrict__ T21) {
   if (threadIdx.x != 0) return;
-  const double hg = h_gric[0];
-  int votes = 0;
-  for (int r = 0; r < R; ++r) votes += (hg > res[TR_EGRIC + r]) ? 1 : 0;
-  const bool valid = (double)votes > (double)R / 2.0;
-  const int best = (int)res[TR_BEST], cheir = best >= 0 ? pinfo[0] : 0;
-  const double* Rt = res + TR_RT;
+  const double hg = h_gric != nullptr ? h_gric[0] : 0.0;
+  if (h_gric != nullptr) {
+    int votes = 0;
+    for (int r = 0; r < R; ++r) votes += (hg > res[DFVO_TAIL_EGRIC + r]) ? 1 : 0;
+    res[DFVO_TAIL_VALID] = ((double)votes > (double)R / 2.0) ? 1.0 : 0.0;
+  }
+  const bool valid = res[DFVO_TAIL_VALID] != 0.0;
+  const int best = (int)res[DFVO_TAIL_BEST], cheir = best >= 0 ? pinfo[0] : 0;
+  const double* Rt = res + DFVO_TAIL_RT;
   const bool pose_ok = valid && best >= 0 && (double)cheir > (double)n * 0.1;
   const double tn = Rt[9] * Rt[9] + Rt[10] * Rt[10] + Rt[11] * Rt[11];
-  const bool gate = pose_ok && tn != 0.0;
-  res[TR_VALID] = valid ? 1.0 : 0.0; res[TR_HGRIC] = hg; res[TR_CHEIR] = (double)cheir; res[TR_GATE] = gate ? 1.0 : 0.0; res[TR_NVALID] = 0.0;
+  res[DFVO_TAIL_HGRIC] = hg; res[DFVO_TAIL_CHEIR] = (double)cheir; res[DFVO_TAIL_GATE] = (pose_ok && tn != 0.0) ? 1.0 : 0.0;
+  res[DFVO_TAIL_NVALID] = 0.0;
   // T_21 = inv([R | t]) = [R^T | -R^T t], rows 0..2
   for (int a = 0; a < 3; ++a) {
     double tt = 0;
@@ -751,7 +799,7 @@ __global__ void __launch_bounds__(128)
 k_scale_points(const double* __restrict__ kp_ref, const double* __restrict__ kp_cur, int n, double fx, double fy, double cx, double cy,
                const double* __restrict__ T21, const float* __restrict__ depth, int H, int W, const double* __restrict__ res,
                double* __restrict__ zbuf, double* __restrict__ dbuf, unsigned long long* __restrict__ keys) {
-  if (res[TR_GATE] == 0.0) return;
+  if (res[DFVO_TAIL_GATE] == 0.0) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   double Pm[3][4];
@@ -780,7 +828,7 @@ k_scale_chain(const unsigned long long* __restrict__ keys, int n, double* __rest
   __shared__ unsigned long long key[SC_MAX];
   __shared__ int wsum[SC_THREADS / 32];
   __shared__ int total_s;
-  if (res[TR_GATE] == 0.0) return;
+  if (res[DFVO_TAIL_GATE] == 0.0) return;
   const int t = threadIdx.x;
   int P = 1; while (P < n) P <<= 1;
   for (int i = t; i < P; i += SC_THREADS) key[i] = i < n ? keys[i] : ~0ull;
@@ -823,17 +871,22 @@ k_scale_chain(const unsigned long long* __restrict__ keys, int n, double* __rest
   __syncthreads();
   const int base = wsum[t >> 5] + incl - cnt;
   for (int q = 0; q < cnt; ++q) ratio[base + q] = rloc[q];
-  if (t == 0) res[TR_NVALID] = (double)total_s;
+  if (t == 0) res[DFVO_TAIL_NVALID] = (double)total_s;
 }
 
-size_t essential_tail_workspace_bytes(int N) { return (size_t)N * 8 * 4 + (size_t)N * 4 + 9 * 8 + 12 * 8 + 1024; }
+#define TAIL_MAX_R 32
+size_t essential_tail_workspace_bytes(int N) {
+  return (size_t)N * 8 * 4 + (size_t)N * 4 + 9 * 8 + 12 * 8 + (size_t)TAIL_MAX_R * 16 + 1024;
+}
 
 int essential_tail(const double* E, const int32_t* info, const double* gric, int R, const double* kp_cur, const double* kp_ref, int N,
                    double fx, double fy, double cx, double cy, const double* h_gric, const float* depth, int H, int W, int min_samples,
                    int max_trials, double stop_prob, double thr, void* workspace, size_t ws_bytes, double* res, uint8_t* pose_mask,
                    int32_t* pose_info, cudaStream_t s) {
-  DFVO_REQUIRE(E && info && gric && kp_cur && kp_ref && h_gric && depth && workspace && res && pose_mask && pose_info, DFVO_EINVAL, "essential_tail args");
-  DFVO_REQUIRE(R >= 1 && R <= 32 && N >= 1 && N <= SC_MAX && min_samples >= 1 && min_samples <= SR_MAX_SAMPLES, DFVO_EINVAL, "essential_tail: R=%d N=%d", R, N);
+  DFVO_REQUIRE(E && info && (gric || !h_gric) && kp_cur && kp_ref && workspace && res && pose_mask && pose_info, DFVO_EINVAL,
+               "essential_tail args");
+  DFVO_REQUIRE(R >= 1 && R <= TAIL_MAX_R && N >= 1 && N <= SC_MAX && min_samples >= 1 && min_samples <= SR_MAX_SAMPLES, DFVO_EINVAL,
+               "essential_tail: R=%d N=%d", R, N);
   DFVO_REQUIRE(ws_bytes >= essential_tail_workspace_bytes(N), DFVO_EINVAL, "essential_tail workspace too small");
   uint8_t* w = reinterpret_cast<uint8_t*>(workspace);
   auto take = [&](size_t bytes) { uint8_t* p = w; w += (bytes + 127) & ~(size_t)127; return p; };
@@ -844,116 +897,24 @@ int essential_tail(const double* E, const int32_t* info, const double* gric, int
   unsigned long long* keys = (unsigned long long*)take((size_t)N * 8);
   double* E_best = (double*)take(9 * 8);
   double* T21 = (double*)take(12 * 8);
-  DFVO_LAUNCH(k_track_pick, dim3(1), dim3(32), 0, s, info, gric, E, R, res, E_best);
+  int32_t* counts = (int32_t*)take((size_t)TAIL_MAX_R * 16);
+  if (h_gric != nullptr) {
+    DFVO_LAUNCH(k_track_pick, dim3(1), dim3(32), 0, s, info, gric, E, R, res, E_best);
+  } else {
+    DFVO_CUDA(cudaMemsetAsync(counts, 0, (size_t)R * 16, s));
+    DFVO_LAUNCH(k_recover_pose_counts, dim3(cdiv(4 * N, 256), R), dim3(256), 0, s, E, kp_cur, kp_ref, N, fx, cx, cy, 50.0, counts);
+    DFVO_LAUNCH(k_track_pick_flow, dim3(1), dim3(32), 0, s, info, (const int32_t*)counts, E, R, N, res, E_best);
+  }
   DFVO_CUDA(cudaMemsetAsync(pose_info, 0, 5 * sizeof(int32_t), s));
   DFVO_LAUNCH(k_recover_pose_vote, dim3(cdiv(4 * N, 256)), dim3(256), 0, s, (const double*)E_best, kp_cur, kp_ref, N, fx, cx, cy, 50.0, pose_mask, pose_info);
-  DFVO_LAUNCH(k_recover_pose_pick, dim3(cdiv(N, 256)), dim3(256), 0, s, (const double*)E_best, N, res + TR_RT, pose_mask, pose_info);
+  DFVO_LAUNCH(k_recover_pose_pick, dim3(cdiv(N, 256)), dim3(256), 0, s, (const double*)E_best, N, res + DFVO_TAIL_RT, pose_mask, pose_info);
   DFVO_LAUNCH(k_track_gate, dim3(1), dim3(32), 0, s, res, (const int32_t*)pose_info, h_gric, R, N, T21);
-  DFVO_LAUNCH(k_scale_points, dim3(cdiv(N, 128)), dim3(128), 0, s, kp_ref, kp_cur, N, fx, fy, cx, cy, (const double*)T21, depth, H, W,
-              (const double*)res, zbuf, dbuf, keys);
-  DFVO_LAUNCH(k_scale_chain, dim3(1), dim3(SC_THREADS), 0, s, (const unsigned long long*)keys, N, res, (const double*)zbuf, (const double*)dbuf, ratio);
-  DFVO_LAUNCH(k_scale_ransac, dim3(1), dim3(SR_THREADS), 0, s, (const double*)ratio, N, min_samples, max_trials, stop_prob, thr, res, perm,
-              (const double*)(res + TR_NVALID), (const double*)(res + TR_GATE));
-  DFVO_CHECK_LAUNCH();
-  return DFVO_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// The same tail for the flow-magnitude validity check (e_tracker.validity.method 'flow', E_tracker.py:249-257,289-300).  The caller has
-// already taken the gate (mean flow > thre) and drawn the shuffles only when it passed.  Per repeat r:
-//   cnt_r   = cv2.recoverPose(E_r, kp_cur[perm_r], kp_ref[perm_r]).count -- a count over all points, so the permutation drops out
-//   valid_r = cnt_r > 0.1 n;   E_r becomes the best only if inliers_r > best inliers AND cnt_r > 0.05 n
-// then the majority vote sum(valid_r) > R / 2, the final recoverPose on the best E, the cheirality gate and (depth != NULL) the scale
-// chain of essential_tail.  res layout as essential_tail's, except [319] = 0 and [335..335+R) = cnt_r.
-// ------------------------------------------------------------------------------------------------
-// every repeat's four candidate counts in one launch: grid (cdiv(4N, 256), R), counts [R][4] zeroed by the caller
-__global__ void __launch_bounds__(256)
-k_recover_pose_counts(const double* __restrict__ E, const double* __restrict__ p1, const double* __restrict__ p2, int N, double focal,
-                      double cx, double cy, double dist, int32_t* __restrict__ counts) {
-  __shared__ double sR[2][3][3], st[3];
-  __shared__ int cnt[4];
-  const int t = threadIdx.x, r = blockIdx.y;
-  if (t == 0) decompose_essential(E + 9 * r, sR, st);
-  if (t < 4) cnt[t] = 0;
-  __syncthreads();
-  const int g = blockIdx.x * 256 + t, j = g >> 2, k = g & 3;
-  const bool m = j < N && cheirality_ok(sR, st, k, p1, p2, j, focal, cx, cy, dist);
-  const unsigned ballot = __ballot_sync(0xffffffffu, m);
-  const int lane = t & 31;
-  if (lane < 4) {
-    const int c = __popc(ballot & (0x11111111u << lane));
-    if (c) atomicAdd(&cnt[lane], c);
-  }
-  __syncthreads();
-  if (t < 4 && cnt[t]) atomicAdd(&counts[4 * r + t], cnt[t]);
-}
-
-__global__ void k_track_pick_flow(const int32_t* __restrict__ info, const int32_t* __restrict__ counts, const double* __restrict__ E, int R,
-                                  int n, double* __restrict__ res, double* __restrict__ E_best) {
-  if (threadIdx.x != 0) return;
-  int best = -1, best_inl = 0, votes = 0;
-  for (int r = 0; r < R; ++r) {
-    int b = 0;                                                         // recoverPose keeps the first candidate with the most points
-    for (int k = 1; k < 4; ++k) if (counts[4 * r + k] > counts[4 * r + b]) b = k;
-    const int c = counts[4 * r + b];
-    votes += ((double)c > (double)n * 0.1) ? 1 : 0;
-    if (info[4 * r] > best_inl && (double)c > (double)n * 0.05) { best = r; best_inl = info[4 * r]; }
-    res[TR_EGRIC + r] = (double)c;
-    for (int q = 0; q < 4; ++q) res[TR_EGRIC + R + 4 * r + q] = (double)info[4 * r + q];
-  }
-  res[TR_BEST] = (double)best;
-  res[TR_VALID] = ((double)votes > (double)R / 2.0) ? 1.0 : 0.0;
-  for (int q = 0; q < 9; ++q) E_best[q] = best >= 0 ? E[9 * best + q] : ((q % 4 == 0 && q < 8) ? 1.0 : 0.0);
-}
-
-// k_track_gate with the vote already in res[TR_VALID]
-__global__ void k_track_gate_flow(double* __restrict__ res, const int32_t* __restrict__ pinfo, int n, double* __restrict__ T21) {
-  if (threadIdx.x != 0) return;
-  const bool valid = res[TR_VALID] != 0.0;
-  const int best = (int)res[TR_BEST], cheir = best >= 0 ? pinfo[0] : 0;
-  const double* Rt = res + TR_RT;
-  const bool pose_ok = valid && best >= 0 && (double)cheir > (double)n * 0.1;
-  const double tn = Rt[9] * Rt[9] + Rt[10] * Rt[10] + Rt[11] * Rt[11];
-  res[TR_HGRIC] = 0.0; res[TR_CHEIR] = (double)cheir; res[TR_GATE] = (pose_ok && tn != 0.0) ? 1.0 : 0.0; res[TR_NVALID] = 0.0;
-  for (int a = 0; a < 3; ++a) {
-    double tt = 0;
-    for (int b = 0; b < 3; ++b) { T21[4 * a + b] = Rt[3 * b + a]; tt += Rt[3 * b + a] * Rt[9 + b]; }
-    T21[4 * a + 3] = -tt;
-  }
-}
-
-size_t essential_flow_tail_workspace_bytes(int N, int R) { return essential_tail_workspace_bytes(N) + (size_t)R * 16 + 128; }
-
-int essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx, double fy,
-                        double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials, double stop_prob, double thr,
-                        void* workspace, size_t ws_bytes, double* res, uint8_t* pose_mask, int32_t* pose_info, cudaStream_t s) {
-  DFVO_REQUIRE(E && info && kp_cur && kp_ref && workspace && res && pose_mask && pose_info, DFVO_EINVAL, "essential_flow_tail args");
-  DFVO_REQUIRE(R >= 1 && R <= 32 && N >= 1 && N <= SC_MAX && min_samples >= 1 && min_samples <= SR_MAX_SAMPLES, DFVO_EINVAL,
-               "essential_flow_tail: R=%d N=%d", R, N);
-  DFVO_REQUIRE(ws_bytes >= essential_flow_tail_workspace_bytes(N, R), DFVO_EINVAL, "essential_flow_tail workspace too small");
-  uint8_t* w = reinterpret_cast<uint8_t*>(workspace);
-  auto take = [&](size_t bytes) { uint8_t* p = w; w += (bytes + 127) & ~(size_t)127; return p; };
-  double* zbuf = (double*)take((size_t)N * 8);
-  double* dbuf = (double*)take((size_t)N * 8);
-  double* ratio = (double*)take((size_t)N * 8);
-  int32_t* perm = (int32_t*)take((size_t)N * 4);
-  unsigned long long* keys = (unsigned long long*)take((size_t)N * 8);
-  double* E_best = (double*)take(9 * 8);
-  double* T21 = (double*)take(12 * 8);
-  int32_t* counts = (int32_t*)take((size_t)R * 16);
-  DFVO_CUDA(cudaMemsetAsync(counts, 0, (size_t)R * 16, s));
-  DFVO_LAUNCH(k_recover_pose_counts, dim3(cdiv(4 * N, 256), R), dim3(256), 0, s, E, kp_cur, kp_ref, N, fx, cx, cy, 50.0, counts);
-  DFVO_LAUNCH(k_track_pick_flow, dim3(1), dim3(32), 0, s, info, (const int32_t*)counts, E, R, N, res, E_best);
-  DFVO_CUDA(cudaMemsetAsync(pose_info, 0, 5 * sizeof(int32_t), s));
-  DFVO_LAUNCH(k_recover_pose_vote, dim3(cdiv(4 * N, 256)), dim3(256), 0, s, (const double*)E_best, kp_cur, kp_ref, N, fx, cx, cy, 50.0, pose_mask, pose_info);
-  DFVO_LAUNCH(k_recover_pose_pick, dim3(cdiv(N, 256)), dim3(256), 0, s, (const double*)E_best, N, res + TR_RT, pose_mask, pose_info);
-  DFVO_LAUNCH(k_track_gate_flow, dim3(1), dim3(32), 0, s, res, (const int32_t*)pose_info, N, T21);
   if (depth != nullptr) {
     DFVO_LAUNCH(k_scale_points, dim3(cdiv(N, 128)), dim3(128), 0, s, kp_ref, kp_cur, N, fx, fy, cx, cy, (const double*)T21, depth, H, W,
                 (const double*)res, zbuf, dbuf, keys);
     DFVO_LAUNCH(k_scale_chain, dim3(1), dim3(SC_THREADS), 0, s, (const unsigned long long*)keys, N, res, (const double*)zbuf, (const double*)dbuf, ratio);
     DFVO_LAUNCH(k_scale_ransac, dim3(1), dim3(SR_THREADS), 0, s, (const double*)ratio, N, min_samples, max_trials, stop_prob, thr, res, perm,
-                (const double*)(res + TR_NVALID), (const double*)(res + TR_GATE));
+                (const double*)(res + DFVO_TAIL_NVALID), (const double*)(res + DFVO_TAIL_GATE));
   }
   DFVO_CHECK_LAUNCH();
   return DFVO_OK;

@@ -1,5 +1,6 @@
 // Pose-solver launchers (ransac.cu).
 #pragma once
+#include "../../include/dfvo_b200.h"
 #include "common.cuh"
 
 namespace dfvo {
@@ -27,31 +28,26 @@ int pnp_ransac(const double* obj, const double* img, int N, const int32_t* perm,
                double fy, double cx, double cy, double threshold, double prob, void* workspace, size_t ws_bytes, double* rt_out,
                int32_t* info, cudaStream_t s);
 
-// sklearn RANSACRegressor scale fit on the device, walking NumPy's MT19937 stream (ransac.cu::k_scale_ransac).  io: device [4 + 313]
-// doubles = {scale, status, trials, inliers} + key[624], pos as uint32; perm_scratch: device [n] int32
+// sklearn RANSACRegressor scale fit on the device, walking NumPy's MT19937 stream (ransac.cu::k_scale_ransac).  io: device
+// [DFVO_TAIL_SCALE_IO] doubles = {scale, status, trials, inliers} + key[624], pos as uint32; perm_scratch: device [n] int32
 int scale_ransac(const double* ratio, int n, int min_samples, int max_trials, double stop_prob, double thr, double* io, int32_t* perm_scratch,
                  cudaStream_t s);
 
 // fused tail of the E-tracker after essential_ransac (ransac.cu): best repeat -> recoverPose -> validity vote / cheirality gate ->
-// depth ratios -> scale regressor, no host round trip.  res: device [335 + 5 R] doubles (layout in ransac.cu), its [4..316] hold the
-// host generator's MT19937 state on entry.  h_gric: device [1] GRIC of the homography model (the caller orders the stream after it).
+// depth ratios -> scale regressor, no host round trip.  res: device [DFVO_TAIL_EGRIC + 5 R] doubles (DFVO_TAIL_* of dfvo_b200.h), the
+// host generator's MT19937 state at DFVO_TAIL_MT on entry.  h_gric: device [1] GRIC of the homography model (the caller orders the
+// stream after it), or nullptr for e_tracker.validity.method 'flow' (gric unused).  depth == nullptr: no scale recovery.
 size_t essential_tail_workspace_bytes(int N);
 int essential_tail(const double* E, const int32_t* info, const double* gric, int R, const double* kp_cur, const double* kp_ref, int N,
                    double fx, double fy, double cx, double cy, const double* h_gric, const float* depth, int H, int W, int min_samples,
                    int max_trials, double stop_prob, double thr, void* workspace, size_t ws_bytes, double* res, uint8_t* pose_mask,
                    int32_t* pose_info, cudaStream_t s);
-// the same tail for e_tracker.validity.method 'flow': per-repeat recoverPose counts, the flow-mode best-E rule and vote, then as above
-// (depth == nullptr: no scale recovery).  res layout as essential_tail's with [335..335+R) = per-repeat cheirality counts.
-size_t essential_flow_tail_workspace_bytes(int N, int R);
-int essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx, double fy,
-                        double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials, double stop_prob, double thr,
-                        void* workspace, size_t ws_bytes, double* res, uint8_t* pose_mask, int32_t* pose_info, cudaStream_t s);
 
 // fused PnP tracker (pnp.cu): in-image / depth-range filter + order-preserving compaction + unprojection -> obj [m][3], img [m][2],
 // count [1] = m; iK = inv(K) row-major [9] (host memory)
 int pnp_filter(const double* kp_ref, const double* kp_cur, int n, const float* depth, int H, int W, double min_depth, double max_depth,
                const double* iK, double* obj, double* img, int32_t* count, cudaStream_t s);
-// pnp_ransac + best repeat: res [8 + 4 R] = {best, inliers, rvec, tvec, info [R][4]}
+// pnp_ransac + best repeat: res [DFVO_PNP_INFO + 4 R] (DFVO_PNP_* of dfvo_b200.h)
 size_t pnp_tail_workspace_bytes(int N, int R, int iters);
 int pnp_tail(const double* obj, const double* img, int N, const int32_t* perm, int R, const int32_t* subsets, int iters, double fx, double fy,
              double cx, double cy, double threshold, double prob, void* workspace, size_t ws_bytes, double* res, cudaStream_t s);

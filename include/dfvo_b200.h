@@ -209,39 +209,50 @@ int dfvo_essential_ransac(const double* p1, const double* p2, int N, const int32
 int dfvo_cv_subset_stream_host(int count, int model_points, int n_subsets, int32_t* out_host);
 /* The scale fit of find_scale_from_depth (E_tracker.py:618-641): RANSACRegressor(LinearRegression(fit_intercept=False),
  * min_samples, max_trials, stop_probability, residual_threshold).fit(ratio[:, None], ones).estimator_.coef_[0, 0], with the sampling
- * drawn from NumPy's global MT19937 exactly as scikit-learn draws it.  ratio [n] float64 (device).  io (device, 4 + 313 doubles):
- * in: doubles [4..] hold the generator state as 625 uint32 (key[624], pos -- np.random.get_state()[1:3]); out: io[0] = scale,
- * io[1] = 1 (ok) / -1 (no consensus: the reference raises ValueError), io[2] = trials, io[3] = inliers, and the advanced
- * generator state for np.random.set_state().  perm_scratch: device [n] int32. */
+ * drawn from NumPy's global MT19937 exactly as scikit-learn draws it.  ratio [n] float64 (device).  io (device, DFVO_TAIL_SCALE_IO
+ * doubles, offsets DFVO_TAIL_* below): in: the generator state at DFVO_TAIL_MT as 625 uint32 (key[624], pos --
+ * np.random.get_state()[1:3]); out: scale, status 1 (ok) / -1 (no consensus: the reference raises ValueError), trials, inliers,
+ * and the advanced generator state for np.random.set_state().  perm_scratch: device [n] int32. */
 int dfvo_scale_ransac(const double* ratio, int n, int min_samples, int max_trials, double stop_prob, double threshold,
                       double* io, int32_t* perm_scratch, void* stream);
+/* Offsets (in doubles) of the packed result of dfvo_essential_tail: res holds DFVO_TAIL_EGRIC + 5 R doubles.  Its prefix
+ * [0, DFVO_TAIL_SCALE_IO) is the io block of dfvo_scale_ransac. */
+enum {
+  DFVO_TAIL_SCALE = 0,         /* scale of the regressor */
+  DFVO_TAIL_STATUS = 1,        /* 1 fitted, -1 no consensus, -2 fewer than 11 ratios, -3 pose rejected (scale recovery not run) */
+  DFVO_TAIL_TRIALS = 2,        /* regressor trials */
+  DFVO_TAIL_INLIERS = 3,       /* regressor inliers */
+  DFVO_TAIL_MT = 4,            /* MT19937 state as 625 uint32 (key[624], pos) in DFVO_TAIL_MT_DOUBLES doubles */
+  DFVO_TAIL_MT_DOUBLES = 313,
+  DFVO_TAIL_SCALE_IO = 317,    /* size of the dfvo_scale_ransac io block */
+  DFVO_TAIL_BEST = 317,        /* best repeat (-1: none) */
+  DFVO_TAIL_VALID = 318,       /* validity vote */
+  DFVO_TAIL_HGRIC = 319,       /* H_gric (0 for flow validity) */
+  DFVO_TAIL_CHEIR = 320,       /* cheirality count of recoverPose on the best E */
+  DFVO_TAIL_NVALID = 321,      /* valid depth ratios */
+  DFVO_TAIL_GATE = 322,        /* 1: the pose stands and |t| != 0, scale recovery runs */
+  DFVO_TAIL_RT = 323,          /* R (row-major) then t of recoverPose: 12 doubles */
+  DFVO_TAIL_EGRIC = 335        /* [R] E_gric (flow validity: per-repeat cheirality counts), then info [R][4] */
+};
 /* Everything of the hybrid tracker between "the essential-matrix repeats are done" and "pose and scale are known" in one enqueue, no
- * host round trip (dfvo.py:165-193): the first repeat with the most inliers (E_tracker.py:278-281), cv2.recoverPose on its E (:292-300),
- * the validity vote H_gric > E_gric (:286-290), and -- when the pose stands and |t| != 0 -- find_scale_from_depth (:571-643): triangulation
- * of the normalised keypoints with inv([R|t]), CNN depth at int(kp_cur), last-writer-wins per pixel, depth ratios in row-major pixel
- * order, RANSACRegressor with NumPy's generator state (dfvo_scale_ransac).  E [R][9], info [R][4], gric [R]: outputs of
- * dfvo_essential_ransac; h_gric [1]: GRIC of dfvo_homography_ransac (the caller makes the stream wait for it); depth [H][W] float32
- * (pre-processed, dfvo_depth_post).  res (device, 335 + 5 R doubles): in: [4..316] = generator state (625 uint32); out: [0] scale,
- * [1] status (1 fitted, -1 no consensus, -2 fewer than 11 ratios, -3 pose rejected: scale recovery not run, generator untouched),
- * [2] trials, [3] inliers, [4..316] advanced generator state, [317] best repeat, [318] vote, [319] H_gric, [320] cheirality count,
- * [321] valid ratios, [322] gate, [323..334] R|t of recoverPose, [335..) E_gric [R], info [R][4] as doubles.  N <= 4096. */
+ * host round trip (dfvo.py:165-193): the best repeat, cv2.recoverPose on its E (E_tracker.py:292-300), the validity vote, the
+ * cheirality gate and -- when the pose stands and |t| != 0 -- find_scale_from_depth (:571-643): triangulation of the normalised
+ * keypoints with inv([R|t]), CNN depth at int(kp_cur), last-writer-wins per pixel, depth ratios in row-major pixel order,
+ * RANSACRegressor with NumPy's generator state (dfvo_scale_ransac).  E [R][9], info [R][4], gric [R]: outputs of
+ * dfvo_essential_ransac.  The validity method follows h_gric:
+ *   - h_gric != NULL (GRIC, E_tracker.py:270-290): h_gric [1] is the GRIC of dfvo_homography_ransac (the caller makes the stream wait
+ *     for it); the best repeat is the first with the most inliers, the vote is H_gric > E_gric [R].
+ *   - h_gric == NULL (flow, E_tracker.py:182-186,249-257,289-300; called only when the dfvo_flow_mean gate passed): gric is not read.
+ *     Every repeat's cv2.recoverPose(E_r, kp_cur[perm_r], kp_ref[perm_r]) count cnt_r (a count, so independent of the permutation);
+ *     the best repeat is the first with inliers_r > best AND cnt_r > 0.05 N, the vote sum(cnt_r > 0.1 N) > R / 2.
+ * depth [H][W] float32 (pre-processed, dfvo_depth_post), or NULL: pose only -- no scale recovery, [0, DFVO_TAIL_SCALE_IO) untouched.
+ * res (device, DFVO_TAIL_EGRIC + 5 R doubles, offsets above): in: the generator state at DFVO_TAIL_MT; out: everything else and the
+ * advanced generator state.  N <= 4096, R <= 32. */
 size_t dfvo_essential_tail_workspace_bytes(int N);
 int dfvo_essential_tail(const double* E, const int32_t* info, const double* gric, int R, const double* kp_cur, const double* kp_ref, int N,
                         double fx, double fy, double cx, double cy, const double* h_gric, const float* depth, int H, int W,
                         int min_samples, int max_trials, double stop_prob, double threshold, void* workspace, size_t workspace_bytes,
                         double* res, uint8_t* pose_mask, int32_t* pose_info, void* stream);
-/* dfvo_essential_tail for e_tracker.validity.method 'flow' (E_tracker.py:182-186,249-257,289-300), called only when the flow gate
- * (dfvo_flow_mean > thre) passed -- a closed gate draws no shuffle and runs no essential matrix.  In one enqueue: every repeat's
- * cv2.recoverPose(E_r, kp_cur[perm_r], kp_ref[perm_r]) count cnt_r (one launch; a count, so independent of the permutation), the
- * best repeat = the first with inliers_r > best AND cnt_r > 0.05 N, the vote sum(cnt_r > 0.1 N) > R / 2, recoverPose on the best E,
- * the cheirality gate and -- when depth != NULL -- the scale recovery of dfvo_essential_tail.  Arguments and res as
- * dfvo_essential_tail's, except: no homography, res[319] = 0 and res[335..335+R) = cnt_r.  With depth == NULL res[0..316] are
- * left as they were (no generator draw).  N <= 4096, R <= 32. */
-size_t dfvo_essential_flow_tail_workspace_bytes(int N, int R);
-int dfvo_essential_flow_tail(const double* E, const int32_t* info, int R, const double* kp_cur, const double* kp_ref, int N, double fx,
-                             double fy, double cx, double cy, const float* depth, int H, int W, int min_samples, int max_trials,
-                             double stop_prob, double threshold, void* workspace, size_t workspace_bytes, double* res, uint8_t* pose_mask,
-                             int32_t* pose_info, void* stream);
 /* The flow-magnitude gate of the E-tracker (E_tracker.py:182-185): np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1)), bit-equal to
  * NumPy (rounded products and sums, NumPy's pairwise summation order).  kp [n][2] float64 (device).  status: NULL, or the device
  * status of dfvo_local_bestn ({good, n, ...}), which then supplies the count -- so the selection's one status read also carries
@@ -253,9 +264,17 @@ int dfvo_flow_mean(const double* kp_ref, const double* kp_cur, int n, const int3
  * [9] in HOST memory (its off-diagonal zeros are checked).  count (device, 1 int32) = m. */
 int dfvo_pnp_filter(const double* kp_ref, const double* kp_cur, int n, const float* depth, int H, int W, double min_depth,
                     double max_depth, const double* iK_host, double* obj, double* img, int32_t* count, void* stream);
+/* Offsets (in doubles) of the packed result of dfvo_pnp_tail: res holds DFVO_PNP_INFO + 4 R doubles. */
+enum {
+  DFVO_PNP_BEST = 0,           /* best repeat (-1: none) */
+  DFVO_PNP_INLIERS = 1,        /* its RANSAC inliers */
+  DFVO_PNP_RVEC = 2,           /* its rvec [3] */
+  DFVO_PNP_TVEC = 5,           /* its tvec [3] */
+  DFVO_PNP_INFO = 8            /* info [R][4] of dfvo_pnp_ransac */
+};
 /* Second half: dfvo_pnp_ransac on the filtered points (N = m >= 5, perm = the host's R shuffles of arange(m), subsets =
  * dfvo_cv_subset_stream_host(m, 5, iters)) and the best repeat (found && inliers > best, first maximum; pnp_tracker.py:108-110).
- * res (device, 8 + 4 R doubles) = {best (-1: none), inliers, rvec[3], tvec[3], info [R][4]}. */
+ * res (device, DFVO_PNP_INFO + 4 R doubles, offsets above). */
 size_t dfvo_pnp_tail_workspace_bytes(int N, int R, int iters);
 int dfvo_pnp_tail(const double* obj, const double* img, int N, const int32_t* perm, int R, const int32_t* subsets, int iters,
                   double fx, double fy, double cx, double cy, double threshold, double prob, void* workspace,
