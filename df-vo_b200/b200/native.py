@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(CSRC, "libdfvo_b200.so")
 
 PREC_FP32, PREC_BF16, PREC_TF32 = 0, 1, 2
 PREC_NAMES = {"fp32": PREC_FP32, "bf16": PREC_BF16, "tf32": PREC_TF32}
-NET_LITEFLOWNET, NET_MONODEPTH2 = 0, 1
+NET_LITEFLOWNET, NET_MONODEPTH2, NET_POSENET = 0, 1, 2
 ACT_NONE, ACT_LEAKY, ACT_RELU, ACT_ELU, ACT_SIGMOID = 0, 1, 2, 3, 4
 
 # offsets (in doubles) of the packed results of dfvo_essential_tail / dfvo_scale_ransac and dfvo_pnp_tail (the DFVO_TAIL_* and
@@ -78,6 +78,9 @@ SIGNATURES = {
                                       c_void_p, c_void_p]),
     "dfvo_monodepth2_build": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float, c_float]),
     "dfvo_monodepth2_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dfvo_posenet_build": (c_int, [c_void_p, c_int, c_int, c_int, c_float]),
+    "dfvo_posenet_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dfvo_depth_consistency": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dfvo_lanczos_resize_u8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
                                        c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dfvo_depth_post": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_double, c_double, c_float, c_float,
@@ -181,6 +184,12 @@ class Context:
 
     def monodepth2_forward(self, img, depth_out, stream=0):
         self.lib.check(self.lib.dfvo_monodepth2_forward(self.h, img, depth_out, stream))
+
+    def posenet_build(self, feed_h, feed_w, precision=PREC_BF16, baseline_multiplier=5.4):
+        self.lib.check(self.lib.dfvo_posenet_build(self.h, feed_h, feed_w, precision, baseline_multiplier))
+
+    def posenet_forward(self, feed_ref, feed_cur, pose_out, stream=0):
+        self.lib.check(self.lib.dfvo_posenet_forward(self.h, feed_ref, feed_cur, pose_out, stream))
 
     def liteflow_geometry(self):
         a, b, c = c_int(), c_int(), c_int()

@@ -25,10 +25,11 @@ from . import runtime as rt_mod
 class FrameState:
     """Device buffers of one frame: image, depths and (for every frame but the first) the flows of the pair
     (previous frame -> this frame).  `ready` = event recorded after the frame's networks (two-stream mode)."""
-    __slots__ = ("id", "img", "depth", "raw_depth", "fwd", "bwd", "diff", "ready", "img_ready")
+    __slots__ = ("id", "img", "depth", "raw_depth", "fwd", "bwd", "diff", "ready", "img_ready", "feed", "feed_ready", "deep_pose")
 
     def __init__(self):
         self.fwd = self.bwd = self.diff = self.ready = self.img_ready = None
+        self.feed = self.feed_ready = self.deep_pose = None
 
 
 class _ForkJoin:
@@ -83,6 +84,10 @@ class FramePipeline:
             raise ValueError("FramePipeline implements tracking_method 'hybrid' and 'PnP', not %r" % (self.tracking_method,))
         if self.validity not in ("GRIC", "flow"):
             raise ValueError("FramePipeline implements e_tracker.validity.method 'GRIC' and 'flow', not %r" % (self.validity,))
+        # kp_selection.depth_consistency (dfvo.py:84,142-143,338-345): the PoseNet of (ref, cur) masks the selection
+        self.depth_consistency = bool(self.cfg.kp_selection.depth_consistency.enable)
+        if self.depth_consistency and not self.cfg.deep_pose.enable:
+            raise ValueError("kp_selection.depth_consistency needs deep_pose.enable (the PoseNet gives its pose, dfvo.py:338-345)")
         self.K = [float(v) for v in K]
         self.H, self.W = height, width
         self.rt = runtime or rt_mod.get()
@@ -121,10 +126,15 @@ class FramePipeline:
             self.s_trk = self.rt.new_stream(high_priority=True)
 
     # ------------------------------------------------------------------ setup
-    def load_weights(self, flow_weights, depth_enc, depth_dec):
+    def load_weights(self, flow_weights, depth_enc, depth_dec, pose_enc=None, pose_dec=None):
+        """pose_enc / pose_dec: pose_encoder.pth / pose.pth, needed (and only used) with kp_selection.depth_consistency."""
+        if self.depth_consistency and (pose_enc is None or pose_dec is None):
+            raise ValueError("kp_selection.depth_consistency needs the PoseNet weights (pose_enc, pose_dec)")
         for e in self.engs:
             e.build_flow(flow_weights, pairs=1, precision=self.precision)
             e.build_depth(depth_enc, depth_dec, precision=self.precision, dataset=self.cfg.dataset)
+            if self.depth_consistency:
+                e.build_pose(pose_enc, pose_dec, precision=self.precision, dataset=self.cfg.dataset)
 
     def engine_for(self, fid):
         """The network engine of frame `fid` (tracking always uses engine 0's solvers)."""
@@ -174,7 +184,16 @@ class FramePipeline:
         st.raw_depth = self._buf("raw%d" % slot, (self.H, self.W), np.float32)
         st.depth = self._buf("dep%d" % slot, (self.H, self.W), np.float32)
         with self.depth_stream(fid):
-            d = eng.depth(eng.depth_feed(st.img))                        # LANCZOS resize + ToTensor on the device
+            if self.depth_consistency:
+                # the frame keeps its feed: the next frame's PoseNet reads it as the reference image (deep_models.py:218-226)
+                st.feed = eng.depth_feed(st.img, out=self._buf("feed%d" % slot, (1, 3, eng.feed_h, eng.feed_w), np.float32))
+                if self.overlap:
+                    st.feed_ready = self.rt.record_event()
+                d = eng.depth(st.feed)
+                if self.ref is not None:
+                    self.pose_cnn(eng, st, slot)
+            else:
+                d = eng.depth(eng.depth_feed(st.img))                    # LANCZOS resize + ToTensor on the device
             c = self.cfg
             eng.depth_post(d, c.crop.depth_crop, float(c.depth.min_depth), float(c.depth.max_depth), st.raw_depth, st.depth)
         if self.ref is not None:
@@ -184,6 +203,13 @@ class FramePipeline:
         if self.inject is not None:
             self.inject(self, st)
         return st
+
+    def pose_cnn(self, eng, st, slot):
+        """ref_data['deep_pose'] = forward_pose([ref, cur]) (dfvo.py:338-345) on the frame's depth stream, after the reference
+        frame's feed (another engine's stream with inflight > 1) is ready.  The pose stays on the device."""
+        if self.overlap and self.ref.feed_ready is not None:
+            self.rt.wait_event(self.ref.feed_ready)
+        st.deep_pose = eng.pose(self.ref.feed, st.feed, out=self._buf("dpose%d" % slot, (4, 4), np.float32))
 
     def mark_image_ready(self, st):
         """Called by infer() right after the frame's image is on the device (its upload was enqueued on this frame's
@@ -228,7 +254,15 @@ class FramePipeline:
         want_mean = self.tracking_method == "hybrid" and self.validity == "flow" and self.fused_tail
         flow_mean = None
         if b.enable:
-            sel = eng.select_local_bestn(diff, fwd, b.num_row, b.num_col, b.num_bestN, b.thre, with_flow_mean=want_mean)
+            dd, dthre = None, 0.05
+            if self.depth_consistency:                                    # DepthConsistency.compute (dfvo.py:142-143)
+                cx, cy, fx, fy = K
+                Km = np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1]])
+                dd = eng.depth_consistency(cur.raw_depth, ref.raw_depth, cur.deep_pose, Km, np.linalg.inv(Km),
+                                           out=self._buf("ddiff", (self.H, self.W), np.float32))
+                dthre = float(c.kp_selection.depth_consistency.thre)
+            sel = eng.select_local_bestn(diff, fwd, b.num_row, b.num_col, b.num_bestN, b.thre, depth_diff_buf=dd, depth_thre=dthre,
+                                         with_flow_mean=want_mean)
             good, n, kp1_buf, kp2_buf = sel[:4]
             flow_mean = sel[4] if want_mean else None
         else:

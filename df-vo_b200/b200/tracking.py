@@ -21,6 +21,11 @@ def depth_constants(dataset):
     return TUM_DEPTH if "tum" in dataset else KITTI_DEPTH
 
 
+def pose_baseline_multiplier(dataset):
+    """Monodepth2PoseNet.stereo_baseline_multiplier (pose/monodepth2/monodepth2.py:77-84)."""
+    return 5.4 if ("kitti" in dataset or "robotcar" in dataset) else 1.0
+
+
 def shuffles(rng, n, repeat):
     """The reference's per-repeat shuffles (E_tracker.py:225-226, pnp_tracker.py:90-95): `repeat` permutations of arange(n), each
     drawn by rng.shuffle in turn, so the generator advances exactly as in the reference."""
@@ -59,6 +64,7 @@ class Engine:
         self.H, self.W = int(height), int(width)
         self.flow_ready = False
         self.depth_ready = False
+        self.pose_ready = False
         # Workspaces are allocated once per configuration for a CAPACITY of keypoints (grown geometrically if a frame ever
         # exceeds it) and handed out as exactly-shaped views: with local_bestN the keypoint count changes almost every
         # frame, and a per-count cache would grow without bound and put cudaMalloc into the tracked region.
@@ -86,6 +92,38 @@ class Engine:
         self.ctx.monodepth2_build(self.feed_h, self.feed_w, precision, c["min_depth"], c["max_depth"], c["baseline"])
         self.depth_out = self.rt.empty((self.feed_h, self.feed_w), np.float32)
         self.depth_ready = True
+
+    def build_pose(self, enc, dec, precision=native.PREC_BF16, dataset="kitti_odom"):
+        """Monodepth2PoseNet (pose/monodepth2/monodepth2.py:31-84) at the depth network's feed size (deep_models.py:220), so
+        build_depth first.  ``enc``: pose_encoder.pth (only its ``encoder.*`` keys are used), ``dec``: pose.pth."""
+        assert self.depth_ready, "build_depth first: the PoseNet reads the depth network's feeds"
+        self.ctx.load_weights(native.NET_POSENET, {k: v for k, v in enc.items() if k.startswith("encoder.")})
+        self.ctx.load_weights(native.NET_POSENET, dec)
+        self.ctx.posenet_build(self.feed_h, self.feed_w, precision, pose_baseline_multiplier(dataset))
+        self.pose_out = self.rt.empty((4, 4), np.float32)
+        self.pose_ready = True
+
+    def pose(self, feed_ref, feed_cur, out=None):
+        """Monodepth2PoseNet.inference_pose of the depth feeds [ref, cur] (deep_models.py:208-230) -> device fp32 [4,4]."""
+        assert self.pose_ready, "build_pose first"
+        out = out or self.pose_out
+        self.ctx.posenet_forward(feed_ref.ptr, feed_cur.ptr, out.ptr, self.rt.stream_ptr())
+        return out
+
+    def depth_consistency(self, depth_cur, depth_ref, T_buf, K_mat, inv_K_mat, out=None):
+        """DepthConsistency.compute (depth_consistency.py:31-163): [H,W] raw depths of the current / reference frame and the
+        device fp32 4x4 pose -> depth_diff [H,W] (device).  K_mat / inv_K_mat: the 3x3 float64 intrinsics, cast to float32 like
+        the reference."""
+        if out is None:
+            if getattr(self, "_dc_out", None) is None:
+                self._dc_out = self.rt.empty((self.H, self.W), np.float32)
+            out = self._dc_out
+        K32 = np.ascontiguousarray(np.asarray(K_mat, np.float64)[:3, :3], np.float32)
+        iK32 = np.ascontiguousarray(np.asarray(inv_K_mat, np.float64)[:3, :3], np.float32)
+        self.lib.check(self.lib.dfvo_depth_consistency(depth_cur.ptr, depth_ref.ptr, self.H, self.W, T_buf.ptr,
+                                                       K32.ctypes.data_as(ctypes.c_void_p), iK32.ctypes.data_as(ctypes.c_void_p),
+                                                       out.ptr, self.rt.stream_ptr()))
+        return out
 
     def flow(self, img_bufs, out=None):
         """img_bufs: 2*pairs uint8 HWC device buffers [ref0, cur0, ...] -> (fwd, bwd, diff) buffers

@@ -77,10 +77,11 @@ static int run_graphed(GraphCache&, const std::vector<uintptr_t>&, cudaStream_t,
 
 struct dfvo_ctx {
   int device = 0;
-  WeightStore weights[2];
+  WeightStore weights[3];
   LiteFlowNetBase* lfn = nullptr;
   Monodepth2Base* mono = nullptr;
-  GraphCache flow_graphs, depth_graphs;
+  PoseNetBase* pose = nullptr;
+  GraphCache flow_graphs, depth_graphs, pose_graphs;
 };
 
 #define API_BEGIN try {
@@ -203,6 +204,7 @@ int dfvo_destroy(dfvo_ctx* ctx) {
   if (!ctx) return DFVO_OK;
   delete ctx->lfn;
   delete ctx->mono;
+  delete ctx->pose;
   delete ctx;
   return DFVO_OK;
   API_END
@@ -210,7 +212,7 @@ int dfvo_destroy(dfvo_ctx* ctx) {
 
 int dfvo_load_weight(dfvo_ctx* ctx, int net, const char* key, const float* data, const int64_t* shape, int ndim) {
   API_BEGIN
-  DFVO_REQUIRE(ctx && key && data && (net == 0 || net == 1) && ndim >= 0 && ndim <= 4, DFVO_EINVAL, "dfvo_load_weight args");
+  DFVO_REQUIRE(ctx && key && data && net >= 0 && net <= DFVO_NET_POSENET && ndim >= 0 && ndim <= 4, DFVO_EINVAL, "dfvo_load_weight args");
   HostTensor t;
   size_t n = 1;
   for (int i = 0; i < ndim; ++i) { t.shape.push_back(shape[i]); n *= (size_t)shape[i]; }
@@ -353,6 +355,33 @@ int dfvo_monodepth2_forward(dfvo_ctx* ctx, const float* img, float* depth_out, v
   DFVO_REQUIRE(ctx && ctx->mono && img && depth_out, DFVO_ESTATE, "dfvo_monodepth2_forward: call dfvo_monodepth2_build first");
   std::vector<uintptr_t> key = {(uintptr_t)img, (uintptr_t)depth_out};
   return run_graphed(ctx->depth_graphs, key, (cudaStream_t)stream, [&]() { return ctx->mono->run(img, depth_out, (cudaStream_t)stream); });
+  API_END
+}
+
+int dfvo_posenet_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, float baseline_multiplier) {
+  API_BEGIN
+  DFVO_REQUIRE(ctx && precision >= 0 && precision <= 2, DFVO_EINVAL, "dfvo_posenet_build args");
+  DFVO_CUDA(cudaSetDevice(ctx->device));
+  delete ctx->pose;
+  ctx->pose = nullptr;
+  ctx->pose_graphs.clear();
+  return posenet_create(ctx->weights[DFVO_NET_POSENET], feed_h, feed_w, precision, baseline_multiplier, &ctx->pose);
+  API_END
+}
+
+int dfvo_posenet_forward(dfvo_ctx* ctx, const float* feed_ref, const float* feed_cur, float* pose_out, void* stream) {
+  API_BEGIN
+  DFVO_REQUIRE(ctx && ctx->pose && feed_ref && feed_cur && pose_out, DFVO_ESTATE, "dfvo_posenet_forward: call dfvo_posenet_build first");
+  std::vector<uintptr_t> key = {(uintptr_t)feed_ref, (uintptr_t)feed_cur, (uintptr_t)pose_out};
+  return run_graphed(ctx->pose_graphs, key, (cudaStream_t)stream, [&]() { return ctx->pose->run(feed_ref, feed_cur, pose_out, (cudaStream_t)stream); });
+  API_END
+}
+
+int dfvo_depth_consistency(const float* depth_cur, const float* depth_ref, int H, int W, const float* T, const float* K_host,
+                           const float* inv_K_host, float* depth_diff, void* stream) {
+  API_BEGIN
+  DFVO_REQUIRE(depth_cur && depth_ref && T && K_host && inv_K_host && depth_diff && H > 1 && W > 1, DFVO_EINVAL, "dfvo_depth_consistency args");
+  return geom_depth_consistency(depth_cur, depth_ref, H, W, T, K_host, inv_K_host, depth_diff, (cudaStream_t)stream);
   API_END
 }
 

@@ -108,6 +108,53 @@ int disp_to_depth(const float* disp, int n, float min_depth, float max_depth, fl
   return DFVO_OK;
 }
 
+// PoseDecoder.forward after net.3 (pose_decoder.py: out.mean(3).mean(2), 0.01 * view(-1, 2, 1, 6), frame 0), then
+// transformation_from_parameters(axisangle, translation, invert=True) (layers.py:28-94) and pose[:, :3, 3] *= baseline
+// (monodepth2.py:117-118), all in float32 in the torch operation order.  One block: thread (c, y) averages row y of channel c
+// over x, then thread c averages its rows, then thread 0 builds the matrix.
+#define POSE_HEAD_MAXH 64
+__global__ void k_pose_head(const float* __restrict__ out12, int h, int w, int pitch, float baseline, float* __restrict__ pose) {
+  __shared__ float rowmean[6 * POSE_HEAD_MAXH];
+  __shared__ float p6[6];
+  for (int t = threadIdx.x; t < 6 * h; t += blockDim.x) {
+    const int c = t / h, y = t - c * h;
+    float s = 0.f;
+    for (int x = 0; x < w; ++x) s += out12[((size_t)y * w + x) * pitch + c];
+    rowmean[t] = s / (float)w;
+  }
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    float s = 0.f;
+    for (int y = 0; y < h; ++y) s += rowmean[threadIdx.x * h + y];
+    p6[threadIdx.x] = 0.01f * (s / (float)h);
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  // rot_from_axisangle (layers.py:63-94)
+  const float vx = p6[0], vy = p6[1], vz = p6[2];
+  const float angle = sqrtf(vx * vx + vy * vy + vz * vz);
+  const float x = vx / (angle + 1e-7f), y = vy / (angle + 1e-7f), z = vz / (angle + 1e-7f);
+  const float ca = cosf(angle), sa = sinf(angle), C = 1.f - ca;
+  const float xs = x * sa, ys = y * sa, zs = z * sa;
+  const float xC = x * C, yC = y * C, zC = z * C;
+  const float xyC = x * yC, yzC = y * zC, zxC = z * xC;
+  const float R[3][3] = {{x * xC + ca, xyC - zs, zxC + ys}, {xyC + zs, y * yC + ca, yzC - xs}, {zxC - ys, yzC + xs, z * zC + ca}};
+  // invert: M = R^T @ translation(-t)
+  const float t[3] = {-p6[3], -p6[4], -p6[5]};
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) pose[4 * i + j] = R[j][i];
+    pose[4 * i + 3] = (R[0][i] * t[0] + R[1][i] * t[1] + R[2][i] * t[2]) * baseline;
+  }
+  pose[12] = 0.f; pose[13] = 0.f; pose[14] = 0.f; pose[15] = 1.f;
+}
+
+int pose_head(const float* out12, int h, int w, int pitch, float baseline_multiplier, float* pose_out, cudaStream_t s) {
+  DFVO_REQUIRE(h >= 1 && h <= POSE_HEAD_MAXH && w >= 1 && pitch >= 12, DFVO_ESHAPE, "pose_head: %dx%d map (at most %d rows)", h, w, POSE_HEAD_MAXH);
+  DFVO_LAUNCH(k_pose_head, dim3(1), dim3(128), 0, s, out12, h, w, pitch, baseline_multiplier, pose_out);
+  DFVO_CHECK_LAUNCH();
+  return DFVO_OK;
+}
+
 // cv2.resize(..., INTER_NEAREST) (OpenCV resizeNN): inv_scale = W / w, ifx = 1 / inv_scale,
 // sx = min(floor(dx * ifx), w - 1), all in double -- note 1/(W/w) is not bit-identical to w/W
 __global__ void k_depth_post(const float* __restrict__ depth, int h, int w, int H, int W, int y0, int y1, int x0, int x1,

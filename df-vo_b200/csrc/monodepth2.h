@@ -1,4 +1,5 @@
-// monodepth2 (ResNet-18 encoder + skip decoder) depth runner (implementation: monodepth2.cu).
+// monodepth2 depth runner (ResNet-18 encoder + skip decoder) and PoseNet runner (the same encoder with a 6-channel stem +
+// PoseDecoder) (implementation: monodepth2.cu).
 #pragma once
 #include "net_common.h"
 
@@ -15,5 +16,16 @@ struct Monodepth2Base {
 
 int monodepth2_create(const WeightStore& ws, int feed_h, int feed_w, int precision, float min_depth, float max_depth,
                       float baseline, Monodepth2Base** out);
+
+struct PoseNetBase {
+  virtual ~PoseNetBase() {}
+  // feed_ref / feed_cur: float NCHW [1,3,h,w] in [0,1] (the depth network's feeds, deep_models.py:218-226);
+  // pose_out: device fp32 4x4 row-major = Monodepth2PoseNet.inference_pose([ref, cur])[0] (pose/monodepth2/monodepth2.py:102-119)
+  virtual int run(const float* feed_ref, const float* feed_cur, float* pose_out, cudaStream_t s) = 0;
+  virtual void geometry(int* h, int* w) = 0;
+  virtual size_t bytes() = 0;
+};
+
+int posenet_create(const WeightStore& ws, int feed_h, int feed_w, int precision, float baseline_multiplier, PoseNetBase** out);
 
 }  // namespace dfvo

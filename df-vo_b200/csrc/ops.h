@@ -141,6 +141,10 @@ template <typename T>
 int upcat_reflect(Ten<const T> lo, int up, Ten<const T> skip, Ten<T> out, cudaStream_t s);
 // sigmoid disparity -> depth (layers.py:16-25, monodepth2.py:111-138): depth = baseline / (min_disp + (max_disp-min_disp)*disp)
 int disp_to_depth(const float* disp, int n, float min_depth, float max_depth, float baseline, float* depth, cudaStream_t s);
+// PoseDecoder tail + transformation_from_parameters(invert=True) (pose_decoder.py, layers.py:28-94, monodepth2.py:102-119):
+// out12 [h][w][pitch] fp32 (channels 0..11 of net.3) -> spatial mean, x 0.01, frame 0's axis-angle / translation, 4x4 pose with
+// the translation times baseline_multiplier -> pose_out (device fp32 [4][4])
+int pose_head(const float* out12, int h, int w, int pitch, float baseline_multiplier, float* pose_out, cudaStream_t s);
 // cv2.resize(INTER_NEAREST) to (W,H) + preprocess_depth (dfvo.py:314-319, utils.py:89-114)
 int depth_post(const float* depth, int h, int w, int H, int W, double crop_y0, double crop_y1, double crop_x0, double crop_x1,
                float min_depth, float max_depth, float* raw_out, float* depth_out, cudaStream_t s);
@@ -176,6 +180,10 @@ int geom_project(const float* points, int H, int W, const double* K12, float eps
 // mode 0: xy [H][W][2] (Reprojection.forward);  mode 1: planar flow [2][H][W] (RigidFlow.forward)
 int geom_reproject(const float* depth, int H, int W, const double* T16, const double* K12, const double* iK9, float eps, int normalized,
                    int mode, float* out, cudaStream_t s);
+// DepthConsistency.compute (depth_consistency.py:69-163): depth_diff [H][W] of depth_cur / depth_ref [H][W] under the device fp32
+// pose T [4][4]; K9 / iK9 host float32 3x3 row-major
+int geom_depth_consistency(const float* depth_cur, const float* depth_ref, int H, int W, const float* T, const float* K9, const float* iK9,
+                           float* out, cudaStream_t s);
 // idx: [ncells*n_best] slots (cell-major); cell_counts may be null (all slots valid, e.g. bestN with ncells=1)
 int gather_keypoints(const int32_t* idx, const int32_t* cell_counts, int ncells, int n_best, const float* flow_fwd, int H, int W,
                      double* kp1, double* kp2, int32_t* n_out, cudaStream_t s);

@@ -1,8 +1,8 @@
 """``DeepModel`` facade with the reference's interface (libs/deep_models/deep_models.py:25-350), backed by
 the dfvo_b200 CUDA library: LiteFlowNet forward+backward flow with the forward-backward consistency map,
-and monodepth2 single-view depth.  Inference only -- the online-finetuning half of the reference class
-(``setup_train``, ``finetune``, ``save_model``) and the experimental PoseNet are outside the hot path
-(SURVEY.md section 2, rows 1/5/6) and raise ``NotImplementedError``.
+monodepth2 single-view depth and the monodepth2 PoseNet (deep_pose).  Inference only -- the online-finetuning half of the
+reference class (``setup_train``, ``finetune``, ``save_model``) is outside the hot path (SURVEY.md section 2, rows 1/6) and
+raises ``NotImplementedError``.
 """
 import os
 
@@ -62,7 +62,21 @@ class DeepModel:
         if self.cfg.depth.depth_src is None:
             assert self.cfg.depth.deep_depth.pretrained_model is not None, "No precomputed depths nor pretrained depth model"
             self.depth = self.initialize_deep_depth_model()
-        assert not self.cfg.deep_pose.enable, "deep_pose (PoseNet) is outside the dfvo_b200 hot path"
+        if self.cfg.deep_pose.enable:
+            self.pose = self.initialize_deep_pose_model()
+
+    def initialize_deep_pose_model(self):
+        """deep_models.py:104-117 / pose/monodepth2/monodepth2.py:31-84: pose_encoder.pth (the encoder's keys only) + pose.pth, at
+        the depth network's feed size."""
+        assert self.cfg.depth.depth_src is None, "the PoseNet reads the depth network's feed size (deep_models.py:220)"
+        wdir = self.cfg.deep_pose.pretrained_model
+        print("==> Initialize Pose-CNN with [{}]".format(wdir))
+        enc = _load_state_dict(os.path.join(wdir, "pose_encoder.pth"))
+        dec = _load_state_dict(os.path.join(wdir, "pose.pth"))
+        self.engine.build_pose(enc, dec, precision=self.precision, dataset=self.cfg.dataset)
+        h = _DepthHandle()
+        h.stereo_baseline_multiplier = tracking.pose_baseline_multiplier(self.cfg.dataset)
+        return h
 
     def initialize_deep_flow_model(self):
         assert self.cfg.deep_flow.network == "liteflow", "Invalid flow network [{}] is provided.".format(self.cfg.deep_flow.network)
@@ -136,7 +150,20 @@ class DeepModel:
         return out.numpy()
 
     def forward_pose(self, imgs):
-        raise NotImplementedError("deep_pose (PoseNet) is outside the dfvo_b200 hot path (SURVEY.md section 2 row 5)")
+        """deep_models.py:208-230: [ref, cur] uint8 images -> float32 [4,4] pose (relative pose from cur to ref).  The feeds are
+        the device LANCZOS resize of forward_depth (deep_models.py:218-221 resize to the depth network's feed size)."""
+        if not hasattr(self, "_pose_feeds"):
+            shape = (1, 3, self.engine.feed_h, self.engine.feed_w)
+            self._pose_feeds = [self.rt.empty(shape, np.float32), self.rt.empty(shape, np.float32)]
+            self._pose_prev = None                            # host copy of the last call's cur image (its feed is _pose_feeds[1])
+        ref, cur = (np.ascontiguousarray(im, np.uint8) for im in imgs)
+        if self._pose_prev is not None and _same_image(ref, self._pose_prev):
+            self._pose_feeds.reverse()                        # the driver's ref is the previous call's cur: reuse its feed
+        else:
+            self.engine.depth_feed(self.rt.from_host(ref), out=self._pose_feeds[0])
+        self.engine.depth_feed(self.rt.from_host(cur), out=self._pose_feeds[1])
+        self._pose_prev = cur.copy()
+        return self.engine.pose(*self._pose_feeds).numpy().astype(np.float32)
 
     def finetune(self, *a, **k):
         raise NotImplementedError("online finetuning is outside the dfvo_b200 hot path")

@@ -33,12 +33,13 @@ def local_bestN(kp1, kp2, ref_data, cfg, outputs):
     accepted for signature compatibility and ignored -- the kernel derives them from the flow."""
     b = cfg.kp_selection.local_bestN
     assert b.score_method == "flow", "dfvo_b200 implements local_bestN score_method 'flow' (the default)"
-    assert not cfg.kp_selection.depth_consistency.enable, "depth_consistency needs PoseNet (outside the hot path)"
     eng = tracking.default_engine()
     fd = ref_data["flow_diff"]
     assert (fd.shape[0], fd.shape[1]) == (eng.H, eng.W)
+    dc = cfg.kp_selection.depth_consistency
+    dd = _dev(ref_data["depth_diff"], np.float32) if dc.enable else None          # kp_selection.py:118-148
     good, n, k1, k2 = eng.select_local_bestn(_dev(fd, np.float32), _dev(ref_data["flow"], np.float32), b.num_row, b.num_col,
-                                             b.num_bestN, b.thre)
+                                             b.num_bestN, b.thre, dd, float(dc.thre) if dc.enable else 0.05)
     return _finish(outputs, good, n, k1, k2, ref_data)
 
 

@@ -33,6 +33,7 @@ extern "C" {
 
 #define DFVO_NET_LITEFLOWNET 0
 #define DFVO_NET_MONODEPTH2 1
+#define DFVO_NET_POSENET 2     /* pose_encoder.pth (encoder.* keys) + pose.pth (net.0 .. net.3) */
 
 #define DFVO_PREC_FP32 0 /* every conv on CUDA cores in fp32 (parity mode)            */
 #define DFVO_PREC_BF16 1 /* bf16 activations, wgmma tensor-core convs, fp32 accum     */
@@ -67,7 +68,8 @@ int dfvo_destroy(dfvo_ctx* ctx);
 
 /* ---- weights --------------------------------------------------------------------------------
  * Replaces torch.load + load_state_dict: LiteFlow.initialize_network_model (lite_flow.py:31-53)
- * and Monodepth2DepthNet.initialize_network_model (monodepth2.py:29-71).  `key` is the reference
+ * Monodepth2DepthNet.initialize_network_model (monodepth2.py:29-71) and Monodepth2PoseNet.initialize_network_model
+ * (pose/monodepth2/monodepth2.py:31-84).  `key` is the reference
  * state-dict key (e.g. "moduleFeatures.moduleOne.0.weight", "encoder.layer1.0.conv1.weight",
  * "decoder.0.conv.conv.weight"); data_host is fp32, C-contiguous. */
 int dfvo_load_weight(dfvo_ctx* ctx, int net, const char* key, const float* data_host,
@@ -94,6 +96,22 @@ int dfvo_monodepth2_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, 
 /* img: float [1,3,feed_h,feed_w] in [0,1] (the PIL-LANCZOS-resized ToTensor image, deep_models.py:195-201);
  * depth_out [feed_h,feed_w] fp32 = Monodepth2DepthNet.inference_depth (monodepth2.py:121-139). */
 int dfvo_monodepth2_forward(dfvo_ctx* ctx, const float* img, float* depth_out, void* stream);
+/* ---- monodepth2 PoseNet: DeepModel.forward_pose (deep_models.py:208-230) -------------------------------------------------
+ * ResnetEncoder(18, False, 2) + PoseDecoder (pose/monodepth2/monodepth2.py:44-119, pose_decoder.py) from the DFVO_NET_POSENET
+ * weights.  The feed size is the DEPTH network's (deep_models.py:220: self.depth.feed_width/height); baseline_multiplier is
+ * stereo_baseline_multiplier (monodepth2.py:77-84: 5.4 for kitti / robotcar, 1 otherwise). */
+int dfvo_posenet_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, float baseline_multiplier);
+/* feed_ref / feed_cur: float [1,3,feed_h,feed_w] in [0,1] (the feeds of dfvo_lanczos_resize_u8, concatenated [ref, cur] as in
+ * deep_models.py:218-226); pose_out: device fp32 [4][4] row-major = inference_pose(...)[0]: transformation_from_parameters(
+ * axisangle, translation, invert=True) (layers.py:28-94) with the translation times baseline_multiplier (monodepth2.py:102-119). */
+int dfvo_posenet_forward(dfvo_ctx* ctx, const float* feed_ref, const float* feed_cur, float* pose_out, void* stream);
+/* DepthConsistency.compute (depth_consistency.py:31-163): depth_diff [H,W] = clamp(|warp - reproj| / reproj, 0, 1) where reproj is
+ * the depth of depth_cur's points under T and warp = grid_sample(depth_ref, Reprojection(depth_cur, T, K, inv_K),
+ * padding_mode="border", align_corners=True).  depth_cur / depth_ref: the [H,W] NEAREST-resized raw depths (not range-clamped);
+ * T: DEVICE fp32 [4][4] (dfvo_posenet_forward's pose_out, ref_data['deep_pose']); K_host / inv_K_host: float32 3x3 row-major
+ * (cam_intrinsics.mat / inv_mat cast to float32).  A 0/0 ratio stays NaN (it fails the selection's `< thre` test). */
+int dfvo_depth_consistency(const float* depth_cur, const float* depth_ref, int H, int W, const float* T, const float* K_host,
+                           const float* inv_K_host, float* depth_diff, void* stream);
 /* PIL.Image.resize((out_w,out_h), LANCZOS) + transforms.ToTensor (deep_models.py:195-198) on the device,
  * bit-exact with Pillow's 8-bit path.  img uint8 [H,W,3]; bounds_* [out][2] / kk_* [out][ksize] int32 are the
  * fixed-point filter tables of b200/lanczos.py (device memory); tmp uint8 [H][out_w][3]; out_u8 [out_h][out_w][3]

@@ -197,6 +197,35 @@ def monodepth2_weights(seed=4869, height=192, width=640):
     return enc, dec
 
 
+def posenet_weights(seed=5171):
+    """monodepth2 PoseNet: ResnetEncoder(18, False, 2) (6-channel stem) + PoseDecoder(num_ch_enc, 1, 2) (pose_decoder.py:
+    net.0 squeeze 1x1 512->256, net.1 / net.2 3x3 256->256, net.3 1x1 256->12), Kaiming-scaled like monodepth2_weights.
+    Returns (pose_encoder_dict, pose_decoder_dict)."""
+    enc_s, _ = monodepth2_shapes()
+    enc_s["encoder.conv1.weight"] = ("weight", (64, 6, 7, 7))
+    dec_s = {"net.0.weight": ("weight", (256, 512, 1, 1)), "net.0.bias": ("bias", (256,)),
+             "net.1.weight": ("weight", (256, 256, 3, 3)), "net.1.bias": ("bias", (256,)),
+             "net.2.weight": ("weight", (256, 256, 3, 3)), "net.2.bias": ("bias", (256,)),
+             "net.3.weight": ("weight", (12, 256, 1, 1)), "net.3.bias": ("bias", (12,))}
+    rs = np.random.RandomState(seed)
+    out = []
+    for spec in (enc_s, dec_s):
+        d = {}
+        for name, (kind, shp) in spec.items():
+            if kind == "weight":
+                d[name] = (rs.standard_normal(shp) * math.sqrt(2.0 / (shp[1] * shp[2] * shp[3]))).astype(np.float32)
+            elif kind == "bias":
+                d[name] = (rs.standard_normal(shp) * 0.05).astype(np.float32)
+            elif kind == "running_mean":
+                d[name] = (rs.standard_normal(shp) * 0.1).astype(np.float32)
+            elif kind == "running_var":
+                d[name] = rs.uniform(0.5, 1.5, shp).astype(np.float32)
+            else:
+                d[name] = rs.uniform(0.5, 1.0, shp).astype(np.float32)
+        out.append(d)
+    return out[0], out[1]
+
+
 # ----------------------------------------------------------------------------------------
 # Frames, camera, flow / depth / correspondences
 # ----------------------------------------------------------------------------------------
