@@ -80,6 +80,10 @@ SIGNATURES = {
     "dfvo_monodepth2_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "dfvo_posenet_build": (c_int, [c_void_p, c_int, c_int, c_int, c_float]),
     "dfvo_posenet_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dfvo_monodepth2_build_batch": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_float]),
+    "dfvo_monodepth2_forward_batch": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_int, c_void_p, c_void_p]),
+    "dfvo_posenet_build_batch": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float]),
+    "dfvo_posenet_forward_batch": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_int, c_void_p, c_void_p]),
     "dfvo_depth_consistency": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dfvo_lanczos_resize_u8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
                                        c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -190,6 +194,22 @@ class Context:
 
     def posenet_forward(self, feed_ref, feed_cur, pose_out, stream=0):
         self.lib.check(self.lib.dfvo_posenet_forward(self.h, feed_ref, feed_cur, pose_out, stream))
+
+    def monodepth2_build_batch(self, feed_h, feed_w, batch, precision=PREC_BF16, min_depth=0.1, max_depth=100.0, baseline=5.4):
+        self.lib.check(self.lib.dfvo_monodepth2_build_batch(self.h, feed_h, feed_w, batch, precision, min_depth, max_depth, baseline))
+
+    def monodepth2_forward_batch(self, feed_ptrs, depth_out, stream=0):
+        """feed_ptrs: one device address per batch entry."""
+        arr = (c_void_p * len(feed_ptrs))(*feed_ptrs)
+        self.lib.check(self.lib.dfvo_monodepth2_forward_batch(self.h, arr, len(feed_ptrs), depth_out, stream))
+
+    def posenet_build_batch(self, feed_h, feed_w, batch, precision=PREC_BF16, baseline_multiplier=5.4):
+        self.lib.check(self.lib.dfvo_posenet_build_batch(self.h, feed_h, feed_w, batch, precision, baseline_multiplier))
+
+    def posenet_forward_batch(self, feed_ptrs, pose_out, stream=0):
+        """feed_ptrs: 2n device addresses [ref0, cur0, ref1, cur1, ...]."""
+        arr = (c_void_p * len(feed_ptrs))(*feed_ptrs)
+        self.lib.check(self.lib.dfvo_posenet_forward_batch(self.h, arr, len(feed_ptrs) // 2, pose_out, stream))
 
     def liteflow_geometry(self):
         a, b, c = c_int(), c_int(), c_int()

@@ -453,6 +453,12 @@ class FramePipeline:
         return pose
 
     # ------------------------------------------------------------------ driver step
+    def advance(self, cur, ref):
+        """Track the FrameState `cur` against `ref` (None: `cur` starts the sequence), chain the global pose and record
+        ``poses[cur.id]`` / ``modes[cur.id]``; returns the global pose.  For callers that run the networks themselves and only
+        use this pipeline as the tracker of one sequence (multiseq.SequenceBatch); runs on the current stream."""
+        return self._advance(cur, ref)
+
     def _advance(self, cur, ref):
         """Track `cur` against `ref` and chain the global pose (dfvo.py:358-403 loop body)."""
         return self._advance_finish(self._advance_launch(cur, ref))

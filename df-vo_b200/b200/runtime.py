@@ -34,10 +34,18 @@ class Buf:
         self.rt.upload(self, arr)
         return self
 
-    def view(self, shape):
-        """A Buf over the first prod(shape) elements of this buffer (no copy): capacity-allocated workspaces hand out
-        exactly-shaped views so a changing keypoint count never reallocates."""
-        return self.rt.view(self, shape)
+    def view(self, shape, offset=0):
+        """A Buf over prod(shape) elements of this buffer starting at element `offset` (no copy): capacity-allocated workspaces
+        hand out exactly-shaped views so a changing keypoint count never reallocates, and one entry of a batched output
+        (e.g. ``flow_fwd.view((1, 2, H, W), i * 2 * H * W)``) is handed out as a buffer of its own."""
+        if not offset:
+            return self.rt.view(self, shape)
+        n = int(np.prod(shape)) if len(shape) else 1
+        if offset < 0 or offset + n > self.size:
+            raise ValueError("view of %d elements at offset %d exceeds a buffer of %d" % (n, offset, self.size))
+        # the runtime's view takes the leading elements: hand it the (contiguous) tail that starts at `offset`
+        tail = Buf(self.t.reshape(-1)[offset:], (self.size - offset,), self.dtype, self.rt)
+        return self.rt.view(tail, shape)
 
     def clone(self):
         """Device-side copy (same stream as the producer: ordered after it)."""

@@ -84,23 +84,27 @@ class Engine:
         self.flow_diff = self.rt.empty((pairs, self.H, self.W), np.float32)
         self.flow_ready = True
 
-    def build_depth(self, enc, dec, precision=native.PREC_BF16, dataset="kitti_odom"):
+    def build_depth(self, enc, dec, precision=native.PREC_BF16, dataset="kitti_odom", batch=1):
+        """monodepth2 for `batch` feeds per forward (batch > 1: :meth:`depth_batch`, output [batch, feed_h, feed_w])."""
         self.ctx.load_weights(native.NET_MONODEPTH2, enc)
         self.ctx.load_weights(native.NET_MONODEPTH2, dec)
         self.feed_h, self.feed_w = int(enc["height"]), int(enc["width"])
         c = depth_constants(dataset)
-        self.ctx.monodepth2_build(self.feed_h, self.feed_w, precision, c["min_depth"], c["max_depth"], c["baseline"])
-        self.depth_out = self.rt.empty((self.feed_h, self.feed_w), np.float32)
+        self.ctx.monodepth2_build_batch(self.feed_h, self.feed_w, batch, precision, c["min_depth"], c["max_depth"], c["baseline"])
+        self.depth_batch_size = batch
+        self.depth_out = self.rt.empty((self.feed_h, self.feed_w) if batch == 1 else (batch, self.feed_h, self.feed_w), np.float32)
         self.depth_ready = True
 
-    def build_pose(self, enc, dec, precision=native.PREC_BF16, dataset="kitti_odom"):
+    def build_pose(self, enc, dec, precision=native.PREC_BF16, dataset="kitti_odom", batch=1):
         """Monodepth2PoseNet (pose/monodepth2/monodepth2.py:31-84) at the depth network's feed size (deep_models.py:220), so
-        build_depth first.  ``enc``: pose_encoder.pth (only its ``encoder.*`` keys are used), ``dec``: pose.pth."""
+        build_depth first.  ``enc``: pose_encoder.pth (only its ``encoder.*`` keys are used), ``dec``: pose.pth.  batch > 1:
+        `batch` feed pairs per forward (:meth:`pose_batch`, output [batch, 4, 4])."""
         assert self.depth_ready, "build_depth first: the PoseNet reads the depth network's feeds"
         self.ctx.load_weights(native.NET_POSENET, {k: v for k, v in enc.items() if k.startswith("encoder.")})
         self.ctx.load_weights(native.NET_POSENET, dec)
-        self.ctx.posenet_build(self.feed_h, self.feed_w, precision, pose_baseline_multiplier(dataset))
-        self.pose_out = self.rt.empty((4, 4), np.float32)
+        self.ctx.posenet_build_batch(self.feed_h, self.feed_w, batch, precision, pose_baseline_multiplier(dataset))
+        self.pose_batch_size = batch
+        self.pose_out = self.rt.empty((4, 4) if batch == 1 else (batch, 4, 4), np.float32)
         self.pose_ready = True
 
     def pose(self, feed_ref, feed_cur, out=None):
@@ -108,6 +112,17 @@ class Engine:
         assert self.pose_ready, "build_pose first"
         out = out or self.pose_out
         self.ctx.posenet_forward(feed_ref.ptr, feed_cur.ptr, out.ptr, self.rt.stream_ptr())
+        return out
+
+    def pose_batch(self, ref_feeds, cur_feeds, out=None):
+        """:meth:`pose` of pose_batch_size feed pairs (lists of device buffers, any addresses) in one forward -> device fp32
+        [batch, 4, 4]; entry i equals pose(ref_feeds[i], cur_feeds[i])."""
+        assert self.pose_ready, "build_pose first"
+        if len(ref_feeds) != len(cur_feeds):
+            raise ValueError("pose_batch: %d reference feeds, %d current feeds" % (len(ref_feeds), len(cur_feeds)))
+        out = out or self.pose_out
+        ptrs = [p for r, c in zip(ref_feeds, cur_feeds) for p in (r.ptr.value, c.ptr.value)]
+        self.ctx.posenet_forward_batch(ptrs, out.ptr, self.rt.stream_ptr())
         return out
 
     def depth_consistency(self, depth_cur, depth_ref, T_buf, K_mat, inv_K_mat, out=None):
@@ -159,6 +174,14 @@ class Engine:
         assert self.depth_ready, "build_depth first"
         out = out or self.depth_out
         self.ctx.monodepth2_forward(feed_buf.ptr, out.ptr, self.rt.stream_ptr())
+        return out
+
+    def depth_batch(self, feeds, out=None):
+        """:meth:`depth` of depth_batch_size feeds (a list of float32 [1,3,feed_h,feed_w] device buffers, any addresses) in one
+        forward -> depth [batch, feed_h, feed_w]; entry i equals depth(feeds[i])."""
+        assert self.depth_ready, "build_depth first"
+        out = out or self.depth_out
+        self.ctx.monodepth2_forward_batch([f.ptr.value for f in feeds], out.ptr, self.rt.stream_ptr())
         return out
 
     def depth_post(self, depth_buf, crop, min_depth, max_depth, raw_out=None, out=None):

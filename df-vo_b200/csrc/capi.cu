@@ -339,42 +339,75 @@ int dfvo_conv2d(const float* x, const float* w_host, const float* bias_host, flo
   API_END
 }
 
-int dfvo_monodepth2_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, float min_depth, float max_depth, float baseline) {
+int dfvo_monodepth2_build_batch(dfvo_ctx* ctx, int feed_h, int feed_w, int batch, int precision, float min_depth, float max_depth,
+                                float baseline) {
   API_BEGIN
-  DFVO_REQUIRE(ctx && precision >= 0 && precision <= 2, DFVO_EINVAL, "dfvo_monodepth2_build args");
+  DFVO_REQUIRE(ctx && batch >= 1 && precision >= 0 && precision <= 2, DFVO_EINVAL, "dfvo_monodepth2_build args");
   DFVO_CUDA(cudaSetDevice(ctx->device));
   delete ctx->mono;
   ctx->mono = nullptr;
   ctx->depth_graphs.clear();
-  return monodepth2_create(ctx->weights[DFVO_NET_MONODEPTH2], feed_h, feed_w, precision, min_depth, max_depth, baseline, &ctx->mono);
+  return monodepth2_create(ctx->weights[DFVO_NET_MONODEPTH2], feed_h, feed_w, batch, precision, min_depth, max_depth, baseline, &ctx->mono);
+  API_END
+}
+
+int dfvo_monodepth2_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, float min_depth, float max_depth, float baseline) {
+  return dfvo_monodepth2_build_batch(ctx, feed_h, feed_w, 1, precision, min_depth, max_depth, baseline);
+}
+
+// one graph per pointer set: the feeds and the output are baked into the captured launches
+int dfvo_monodepth2_forward_batch(dfvo_ctx* ctx, const float* const* feeds, int n, float* depth_out, void* stream) {
+  API_BEGIN
+  DFVO_REQUIRE(ctx && ctx->mono && feeds && depth_out, DFVO_ESTATE, "dfvo_monodepth2_forward: call dfvo_monodepth2_build first");
+  DFVO_REQUIRE(n == ctx->mono->batch(), DFVO_ESHAPE, "dfvo_monodepth2_forward: %d feeds given, the runner was built for %d", n, ctx->mono->batch());
+  std::vector<uintptr_t> key;
+  for (int i = 0; i < n; ++i) {
+    DFVO_REQUIRE(feeds[i] != nullptr, DFVO_EINVAL, "dfvo_monodepth2_forward: feed %d is null", i);
+    key.push_back((uintptr_t)feeds[i]);
+  }
+  key.push_back((uintptr_t)depth_out);
+  return run_graphed(ctx->depth_graphs, key, (cudaStream_t)stream, [&]() { return ctx->mono->run_batch(feeds, n, depth_out, (cudaStream_t)stream); });
   API_END
 }
 
 int dfvo_monodepth2_forward(dfvo_ctx* ctx, const float* img, float* depth_out, void* stream) {
-  API_BEGIN
   DFVO_REQUIRE(ctx && ctx->mono && img && depth_out, DFVO_ESTATE, "dfvo_monodepth2_forward: call dfvo_monodepth2_build first");
-  std::vector<uintptr_t> key = {(uintptr_t)img, (uintptr_t)depth_out};
-  return run_graphed(ctx->depth_graphs, key, (cudaStream_t)stream, [&]() { return ctx->mono->run(img, depth_out, (cudaStream_t)stream); });
-  API_END
+  return dfvo_monodepth2_forward_batch(ctx, &img, 1, depth_out, stream);
 }
 
-int dfvo_posenet_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, float baseline_multiplier) {
+int dfvo_posenet_build_batch(dfvo_ctx* ctx, int feed_h, int feed_w, int batch, int precision, float baseline_multiplier) {
   API_BEGIN
-  DFVO_REQUIRE(ctx && precision >= 0 && precision <= 2, DFVO_EINVAL, "dfvo_posenet_build args");
+  DFVO_REQUIRE(ctx && batch >= 1 && precision >= 0 && precision <= 2, DFVO_EINVAL, "dfvo_posenet_build args");
   DFVO_CUDA(cudaSetDevice(ctx->device));
   delete ctx->pose;
   ctx->pose = nullptr;
   ctx->pose_graphs.clear();
-  return posenet_create(ctx->weights[DFVO_NET_POSENET], feed_h, feed_w, precision, baseline_multiplier, &ctx->pose);
+  return posenet_create(ctx->weights[DFVO_NET_POSENET], feed_h, feed_w, batch, precision, baseline_multiplier, &ctx->pose);
+  API_END
+}
+
+int dfvo_posenet_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, float baseline_multiplier) {
+  return dfvo_posenet_build_batch(ctx, feed_h, feed_w, 1, precision, baseline_multiplier);
+}
+
+int dfvo_posenet_forward_batch(dfvo_ctx* ctx, const float* const* feeds, int n, float* pose_out, void* stream) {
+  API_BEGIN
+  DFVO_REQUIRE(ctx && ctx->pose && feeds && pose_out, DFVO_ESTATE, "dfvo_posenet_forward: call dfvo_posenet_build first");
+  DFVO_REQUIRE(n == ctx->pose->batch(), DFVO_ESHAPE, "dfvo_posenet_forward: %d feed pairs given, the runner was built for %d", n, ctx->pose->batch());
+  std::vector<uintptr_t> key;
+  for (int i = 0; i < 2 * n; ++i) {
+    DFVO_REQUIRE(feeds[i] != nullptr, DFVO_EINVAL, "dfvo_posenet_forward: feed %d is null", i);
+    key.push_back((uintptr_t)feeds[i]);
+  }
+  key.push_back((uintptr_t)pose_out);
+  return run_graphed(ctx->pose_graphs, key, (cudaStream_t)stream, [&]() { return ctx->pose->run_batch(feeds, n, pose_out, (cudaStream_t)stream); });
   API_END
 }
 
 int dfvo_posenet_forward(dfvo_ctx* ctx, const float* feed_ref, const float* feed_cur, float* pose_out, void* stream) {
-  API_BEGIN
   DFVO_REQUIRE(ctx && ctx->pose && feed_ref && feed_cur && pose_out, DFVO_ESTATE, "dfvo_posenet_forward: call dfvo_posenet_build first");
-  std::vector<uintptr_t> key = {(uintptr_t)feed_ref, (uintptr_t)feed_cur, (uintptr_t)pose_out};
-  return run_graphed(ctx->pose_graphs, key, (cudaStream_t)stream, [&]() { return ctx->pose->run(feed_ref, feed_cur, pose_out, (cudaStream_t)stream); });
-  API_END
+  const float* feeds[2] = {feed_ref, feed_cur};
+  return dfvo_posenet_forward_batch(ctx, feeds, 1, pose_out, stream);
 }
 
 int dfvo_depth_consistency(const float* depth_cur, const float* depth_ref, int H, int W, const float* T, const float* K_host,

@@ -110,10 +110,12 @@ int disp_to_depth(const float* disp, int n, float min_depth, float max_depth, fl
 
 // PoseDecoder.forward after net.3 (pose_decoder.py: out.mean(3).mean(2), 0.01 * view(-1, 2, 1, 6), frame 0), then
 // transformation_from_parameters(axisangle, translation, invert=True) (layers.py:28-94) and pose[:, :3, 3] *= baseline
-// (monodepth2.py:117-118), all in float32 in the torch operation order.  One block: thread (c, y) averages row y of channel c
-// over x, then thread c averages its rows, then thread 0 builds the matrix.
+// (monodepth2.py:117-118), all in float32 in the torch operation order.  One block per batch entry: thread (c, y) averages row y
+// of channel c over x, then thread c averages its rows, then thread 0 builds the matrix.
 #define POSE_HEAD_MAXH 64
 __global__ void k_pose_head(const float* __restrict__ out12, int h, int w, int pitch, float baseline, float* __restrict__ pose) {
+  out12 += (size_t)blockIdx.x * h * w * pitch;
+  pose += 16 * blockIdx.x;
   __shared__ float rowmean[6 * POSE_HEAD_MAXH];
   __shared__ float p6[6];
   for (int t = threadIdx.x; t < 6 * h; t += blockDim.x) {
@@ -148,9 +150,10 @@ __global__ void k_pose_head(const float* __restrict__ out12, int h, int w, int p
   pose[12] = 0.f; pose[13] = 0.f; pose[14] = 0.f; pose[15] = 1.f;
 }
 
-int pose_head(const float* out12, int h, int w, int pitch, float baseline_multiplier, float* pose_out, cudaStream_t s) {
-  DFVO_REQUIRE(h >= 1 && h <= POSE_HEAD_MAXH && w >= 1 && pitch >= 12, DFVO_ESHAPE, "pose_head: %dx%d map (at most %d rows)", h, w, POSE_HEAD_MAXH);
-  DFVO_LAUNCH(k_pose_head, dim3(1), dim3(128), 0, s, out12, h, w, pitch, baseline_multiplier, pose_out);
+int pose_head(const float* out12, int n, int h, int w, int pitch, float baseline_multiplier, float* pose_out, cudaStream_t s) {
+  DFVO_REQUIRE(n >= 1 && h >= 1 && h <= POSE_HEAD_MAXH && w >= 1 && pitch >= 12, DFVO_ESHAPE, "pose_head: %d x %dx%d maps (at most %d rows)", n, h, w,
+               POSE_HEAD_MAXH);
+  DFVO_LAUNCH(k_pose_head, dim3(n), dim3(128), 0, s, out12, h, w, pitch, baseline_multiplier, pose_out);
   DFVO_CHECK_LAUNCH();
   return DFVO_OK;
 }

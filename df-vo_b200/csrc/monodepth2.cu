@@ -12,6 +12,10 @@
 // (depth/monodepth2/layers.py:28-94), translation times stereo_baseline_multiplier.  The encoder is the depth network's
 // (Resnet18Encoder below) with a 6-channel stem.
 //
+// Batch: both runners are built for B images and every layer is one launch over N = B (the coarse encoder / decoder levels
+// alone leave most SMs idle); the per-image arithmetic does not depend on B.  Only the feed normalisation is one launch per
+// image, because every feed is a separate caller buffer.
+//
 // Layout/plan: NHWC; every 3x3 decoder conv reads a reflection-padded buffer produced by one fused
 // "nearest-upsample + concat skip + reflect-pad" kernel, so the convs are plain valid convs and run on
 // the wgmma kernel (T = bf16) or the CUDA-core kernel (T = float, parity mode; stride-2 / 3-channel /
@@ -31,9 +35,9 @@ template <> struct IsBf16m<bf16> { enum { v = 1 }; };
 #define ALLOCM(ptr, type, count) do { ptr = arena.alloc_t<type>(count); if (!ptr) return DFVO_ENOMEM; } while (0)
 
 template <typename T>
-static Ten<T> tv(T* p, int H, int W, int C, int pitch) { return make_ten<T>(p, 1, H, W, C, pitch); }
+static Ten<T> tv(T* p, int N, int H, int W, int C, int pitch) { return make_ten<T>(p, N, H, W, C, pitch); }
 template <typename T>
-static Ten<const T> ctv(const T* p, int H, int W, int C, int pitch) { return cten(make_ten<T>(const_cast<T*>(p), 1, H, W, C, pitch)); }
+static Ten<const T> ctv(const T* p, int N, int H, int W, int C, int pitch) { return cten(make_ten<T>(const_cast<T*>(p), N, H, W, C, pitch)); }
 
 // conv + eval-mode BatchNorm folded into the weights (torchvision BasicBlock / stem)
 template <typename T>
@@ -72,16 +76,16 @@ static int plain_conv(Arena& arena, bool tf32, const WeightStore& ws, const std:
 template <typename T>
 struct Resnet18Encoder {
   bool tf32 = false;          // T = float only: wgmma tf32 convs (DFVO_PREC_TF32)
-  int h = 0, w = 0, cin = 3;
+  int nb = 1, h = 0, w = 0, cin = 3;    // nb: batch (images per run); every buffer below holds nb images
   ConvLayer conv1;
   ConvLayer conv1_tc;          // bf16: the 7x7 stride-2 stem on the tensor cores (see stem_tc_layer)
   bool stem_tc = false;
-  T* imgpad = nullptr;        // [h][w+8][8] column-padded normalised image (zero borders / pad channels)
+  T* imgpad = nullptr;        // [nb][h][w+8][8] column-padded normalised images (zero borders / pad channels)
   struct Block { ConvLayer c1, c2, down; bool has_down = false; int stride = 1; } blk[4][2];
-  T* x0;                      // normalised input NHWC (cin channels, pitch xpitch())
-  T* f[5];                    // encoder features
+  T* x0;                      // normalised input NHWC [nb] (cin channels, pitch xpitch())
+  T* f[5];                    // encoder features [nb]
   int fh[5], fw[5], fc[5];
-  T *pool, *tA, *tB, *tD;     // scratch at layer resolution
+  T *pool, *tA, *tB, *tD;     // scratch at layer resolution [nb]
   unsigned* chain_bars = nullptr;     // arrival counters of the encoder's layer chain
 
   int xpitch() const { return cin == 3 ? 4 : 8; }
@@ -122,8 +126,8 @@ struct Resnet18Encoder {
     return build_conv_layer(arena, wr, nullptr, {{64, 64}, {64, 64}}, 1, 2, 0, 0, true, false, scale.data(), shift.data(), &conv1_tc, 2);
   }
 
-  int build_layers(Arena& arena, const WeightStore& ws, int feed_h, int feed_w, int in_ch) {
-    h = feed_h; w = feed_w; cin = in_ch;
+  int build_layers(Arena& arena, const WeightStore& ws, int batch, int feed_h, int feed_w, int in_ch) {
+    nb = batch; h = feed_h; w = feed_w; cin = in_ch;
     TRYM(bn_conv<T>(arena, tf32, ws, "encoder.conv1", "encoder.bn1", cin, 2, 3, false, &conv1));
     {
       const char* e = getenv("DFVO_MONO_STEM_TC");
@@ -154,10 +158,10 @@ struct Resnet18Encoder {
   }
 
   int alloc_buffers(Arena& arena) {
-    ALLOCM(x0, T, (size_t)h * w * xpitch());
-    ALLOCM(imgpad, T, stem_tc ? (size_t)h * (w + 8) * 8 + 64 : 64);
-    for (int i = 0; i < 5; ++i) ALLOCM(f[i], T, (size_t)fh[i] * fw[i] * fc[i]);
-    const size_t big = (size_t)fh[1] * fw[1] * 64;      // largest BasicBlock tensor (layer1)
+    ALLOCM(x0, T, (size_t)nb * h * w * xpitch());
+    ALLOCM(imgpad, T, stem_tc ? (size_t)nb * h * (w + 8) * 8 + 64 : 64);
+    for (int i = 0; i < 5; ++i) ALLOCM(f[i], T, (size_t)nb * fh[i] * fw[i] * fc[i]);
+    const size_t big = (size_t)nb * fh[1] * fw[1] * 64;      // largest BasicBlock tensor (layer1)
     ALLOCM(pool, T, big); ALLOCM(tA, T, big); ALLOCM(tB, T, big); ALLOCM(tD, T, big);
     return DFVO_OK;
   }
@@ -165,39 +169,43 @@ struct Resnet18Encoder {
   int basic_block(Block& B, const T* in, int ih, int iw, int ic, T* out, int oc, cudaStream_t s) {
     const int oh = ih / B.stride, ow = iw / B.stride;
     Ten<const T> none; memset(&none, 0, sizeof(none));
-    TRYM(run_conv<T>(B.c1, ctv(in, ih, iw, ic, ic), tv(tA, oh, ow, oc, oc), ACT_RELU, none, 0, s));
+    TRYM(run_conv<T>(B.c1, ctv(in, nb, ih, iw, ic, ic), tv(tA, nb, oh, ow, oc, oc), ACT_RELU, none, 0, s));
     const T* idt = in;
     if (B.has_down) {
-      TRYM(run_conv<T>(B.down, ctv(in, ih, iw, ic, ic), tv(tD, oh, ow, oc, oc), ACT_NONE, none, 0, s));
+      TRYM(run_conv<T>(B.down, ctv(in, nb, ih, iw, ic, ic), tv(tD, nb, oh, ow, oc, oc), ACT_NONE, none, 0, s));
       idt = tD;
     }
     // out = relu(bn2(conv2(.)) + identity)   (torchvision BasicBlock.forward)
-    TRYM(run_conv<T>(B.c2, ctv(tA, oh, ow, oc, oc), tv(out, oh, ow, oc, oc), ACT_RELU, ctv(idt, oh, ow, oc, oc), 0, s));
+    TRYM(run_conv<T>(B.c2, ctv(tA, nb, oh, ow, oc, oc), tv(out, nb, oh, ow, oc, oc), ACT_RELU, ctv(idt, nb, oh, ow, oc, oc), 0, s));
     return DFVO_OK;
   }
 
-  // imgs: cin / 3 float NCHW [3,h,w] feeds in [0,1]; fills f[0..4]
+  // imgs: nb * cin / 3 float NCHW [3,h,w] feeds in [0,1], image b's feeds at imgs[b * cin / 3 ..]; fills f[0..4]
   int run(const float* const* imgs, cudaStream_t s) {
     Ten<const T> none; memset(&none, 0, sizeof(none));
+    const int per = cin / 3;
     if (stem_tc) {
-      const long long row = (long long)(w + 8) * 8;
-      for (int i = 0; i < cin / 3; ++i) {
-        Ten<T> pv; pv.p = imgpad + 3 * 8 + 3 * i; pv.N = 1; pv.H = h; pv.W = w; pv.C = 3; pv.sW = 8; pv.sH = row; pv.sN = (long long)h * row;
-        TRYM(normalize_nchw_to_nhwc<T>(imgs[i], 1, 3, h, w, 0.45f, 0.225f, pv, s));          // borders / pad channels stay zero
-      }
+      const long long row = (long long)(w + 8) * 8, img = (long long)h * row;
+      for (int b = 0; b < nb; ++b)
+        for (int i = 0; i < per; ++i) {
+          Ten<T> pv; pv.p = imgpad + b * img + 3 * 8 + 3 * i; pv.N = 1; pv.H = h; pv.W = w; pv.C = 3; pv.sW = 8; pv.sH = row; pv.sN = img;
+          TRYM(normalize_nchw_to_nhwc<T>(imgs[b * per + i], 1, 3, h, w, 0.45f, 0.225f, pv, s));     // borders / pad channels stay zero
+        }
       Ten<const T> eo[2];
       for (int par = 0; par < 2; ++par) {
         Ten<const T>& v = eo[par];
-        v.p = imgpad + par * row; v.N = 1; v.H = h / 2; v.W = w / 2; v.C = 64; v.sW = 16; v.sH = 2 * row; v.sN = (long long)h * row;
+        v.p = imgpad + par * row; v.N = nb; v.H = h / 2; v.W = w / 2; v.C = 64; v.sW = 16; v.sH = 2 * row; v.sN = img;
       }
-      TRYM(run_conv_multi<T>(conv1_tc, eo, 2, tv(f[0], fh[0], fw[0], 64, 64), ACT_RELU, 2.0 * fh[0] * fw[0] * 64.0 * (49.0 * cin), s));
+      TRYM(run_conv_multi<T>(conv1_tc, eo, 2, tv(f[0], nb, fh[0], fw[0], 64, 64), ACT_RELU, 2.0 * nb * fh[0] * fw[0] * 64.0 * (49.0 * cin), s));
     } else {
-      for (int i = 0; i < cin / 3; ++i)
-        TRYM(normalize_nchw_to_nhwc<T>(imgs[i], 1, 3, h, w, 0.45f, 0.225f, tv(x0 + 3 * i, h, w, 3, xpitch()), s));
+      const size_t img = (size_t)h * w * xpitch();
+      for (int b = 0; b < nb; ++b)
+        for (int i = 0; i < per; ++i)
+          TRYM(normalize_nchw_to_nhwc<T>(imgs[b * per + i], 1, 3, h, w, 0.45f, 0.225f, tv(x0 + b * img + 3 * i, 1, h, w, 3, xpitch()), s));
       ConvDirect d = {cin, 64, 7, 7, 2, 3, 3, 0, ACT_RELU, conv1.w_direct, conv1.w_pitch, conv1.bias};
-      TRYM((conv_direct<T, T>(d, ctv(x0, h, w, cin, xpitch()), tv(f[0], fh[0], fw[0], 64, 64), none, s)));
+      TRYM((conv_direct<T, T>(d, ctv(x0, nb, h, w, cin, xpitch()), tv(f[0], nb, fh[0], fw[0], 64, 64), none, s)));
     }
-    TRYM(maxpool3x3s2<T>(ctv(f[0], fh[0], fw[0], 64, 64), tv(pool, fh[1], fw[1], 64, 64), s));
+    TRYM(maxpool3x3s2<T>(ctv(f[0], nb, fh[0], fw[0], 64, 64), tv(pool, nb, fh[1], fw[1], 64, 64), s));
     const T* cur = pool;
     int ch = fh[1], cw = fw[1], cc = 64;
     {
@@ -220,22 +228,23 @@ template <typename T>
 struct MonoImpl : public Monodepth2Base {
   Arena arena;
   bool tf32 = false;          // T = float only: wgmma tf32 convs (DFVO_PREC_TF32)
-  int h = 0, w = 0;
+  int nb = 1, h = 0, w = 0;
   float min_depth = 0.1f, max_depth = 100.f, baseline = 5.4f;
   Resnet18Encoder<T> enc;
   ConvLayer up[10], disp0;
-  // buffers
+  // buffers (nb images each)
   T* padbuf;                  // reflection-padded conv input scratch
   T *dA, *dB;                 // decoder activations
   float* disp;
 
-  int build(const WeightStore& ws, int feed_h, int feed_w, float mind, float maxd, float base) {
-    h = feed_h; w = feed_w; min_depth = mind; max_depth = maxd; baseline = base;
+  int build(const WeightStore& ws, int batch, int feed_h, int feed_w, float mind, float maxd, float base) {
+    nb = batch; h = feed_h; w = feed_w; min_depth = mind; max_depth = maxd; baseline = base;
+    DFVO_REQUIRE(nb >= 1, DFVO_EINVAL, "monodepth2 batch must be at least 1 (got %d)", nb);
     // >= 64: the decoder reflection-pads the 1/32-resolution map by one pixel, which needs at least two rows and columns
     // (torch.nn.ReflectionPad2d refuses a 1-pixel map the same way)
     DFVO_REQUIRE(h % 32 == 0 && w % 32 == 0 && h >= 64 && w >= 64, DFVO_ESHAPE, "monodepth2 feed size must be a multiple of 32 and at least 64x64 (got %dx%d)", h, w);
     enc.tf32 = tf32;
-    TRYM(enc.build_layers(arena, ws, h, w, 3));
+    TRYM(enc.build_layers(arena, ws, nb, h, w, 3));
     const int encc[5] = {64, 64, 128, 256, 512}, dec[5] = {16, 32, 64, 128, 256};
     int idx = 0;
     for (int i = 4; i >= 0; --i) {
@@ -261,16 +270,18 @@ struct MonoImpl : public Monodepth2Base {
       if (b2 > pmax) pmax = b2;
     }
     { size_t d = (size_t)(h + 2) * (w + 2) * 16; if (d > pmax) pmax = d; }
-    ALLOCM(padbuf, T, pmax);
-    ALLOCM(dA, T, (size_t)h * w * 16 + (size_t)(h / 2) * (w / 2) * 32); ALLOCM(dB, T, (size_t)h * w * 16 + (size_t)(h / 2) * (w / 2) * 32);
-    ALLOCM(disp, float, (size_t)h * w);
+    ALLOCM(padbuf, T, (size_t)nb * pmax);
+    const size_t dec_act = (size_t)h * w * 16 + (size_t)(h / 2) * (w / 2) * 32;
+    ALLOCM(dA, T, (size_t)nb * dec_act); ALLOCM(dB, T, (size_t)nb * dec_act);
+    ALLOCM(disp, float, (size_t)nb * h * w);
     ALLOCM(enc.chain_bars, unsigned, 4 * CHAIN_BAR_WORDS);
     return DFVO_OK;
   }
 
-  int run(const float* img, float* depth_out, cudaStream_t s) override {
+  int run_batch(const float* const* imgs, int n, float* depth_out, cudaStream_t s) override {
+    DFVO_REQUIRE(n == nb, DFVO_ESHAPE, "monodepth2: %d feeds given, the runner was built for a batch of %d", n, nb);
     Ten<const T> none; memset(&none, 0, sizeof(none));
-    TRYM(enc.run(&img, s));
+    TRYM(enc.run(imgs, s));
     // ---------------- decoder (depth_decoder.py:50-65) ----------------
     const int dec[5] = {16, 32, 64, 128, 256};
     T* const* f = enc.f;
@@ -280,16 +291,16 @@ struct MonoImpl : public Monodepth2Base {
     int idx = 0;
     for (int i = 4; i >= 0; --i) {
       // upconv(i,0): ConvBlock on x
-      TRYM(upcat_reflect<T>(ctv(x, xh, xw, xc, xc), 1, none, tv(padbuf, xh + 2, xw + 2, xc, xc), s));
-      TRYM(run_conv<T>(up[idx], ctv(padbuf, xh + 2, xw + 2, xc, xc), tv(dA, xh, xw, dec[i], dec[i]), ACT_ELU, none, 0, s));
+      TRYM(upcat_reflect<T>(ctv(x, nb, xh, xw, xc, xc), 1, none, tv(padbuf, nb, xh + 2, xw + 2, xc, xc), s));
+      TRYM(run_conv<T>(up[idx], ctv(padbuf, nb, xh + 2, xw + 2, xc, xc), tv(dA, nb, xh, xw, dec[i], dec[i]), ACT_ELU, none, 0, s));
       ++idx;
       // upsample x2, concat skip, upconv(i,1)
       const int sc = i > 0 ? fc[i - 1] : 0;
       Ten<const T> skip = none;
-      if (i > 0) skip = ctv(f[i - 1], fh[i - 1], fw[i - 1], sc, sc);
+      if (i > 0) skip = ctv(f[i - 1], nb, fh[i - 1], fw[i - 1], sc, sc);
       const int nh = 2 * xh, nw = 2 * xw, ncat = dec[i] + sc;
-      TRYM(upcat_reflect<T>(ctv(dA, xh, xw, dec[i], dec[i]), 2, skip, tv(padbuf, nh + 2, nw + 2, ncat, ncat), s));
-      TRYM(run_conv<T>(up[idx], ctv(padbuf, nh + 2, nw + 2, ncat, ncat), tv(dB, nh, nw, dec[i], dec[i]), ACT_ELU, none, 0, s));
+      TRYM(upcat_reflect<T>(ctv(dA, nb, xh, xw, dec[i], dec[i]), 2, skip, tv(padbuf, nb, nh + 2, nw + 2, ncat, ncat), s));
+      TRYM(run_conv<T>(up[idx], ctv(padbuf, nb, nh + 2, nw + 2, ncat, ncat), tv(dB, nb, nh, nw, dec[i], dec[i]), ACT_ELU, none, 0, s));
       ++idx;
       x = dB; xh = nh; xw = nw; xc = dec[i];
       // swap scratch so the next stage does not overwrite its own input
@@ -297,15 +308,16 @@ struct MonoImpl : public Monodepth2Base {
       x = dA;
     }
     // dispconv scale 0: Conv3x3 (reflect) + sigmoid, 16 -> 1
-    TRYM(upcat_reflect<T>(ctv(x, xh, xw, 16, 16), 1, none, tv(padbuf, xh + 2, xw + 2, 16, 16), s));
+    TRYM(upcat_reflect<T>(ctv(x, nb, xh, xw, 16, 16), 1, none, tv(padbuf, nb, xh + 2, xw + 2, 16, 16), s));
     {
       Ten<const float> fnone; memset(&fnone, 0, sizeof(fnone));
-      TRYM(run_conv_f32out<T>(disp0, ctv(padbuf, xh + 2, xw + 2, 16, 16), make_ten<float>(disp, 1, h, w, 1, 1), ACT_SIGMOID, fnone, s));
+      TRYM(run_conv_f32out<T>(disp0, ctv(padbuf, nb, xh + 2, xw + 2, 16, 16), make_ten<float>(disp, nb, h, w, 1, 1), ACT_SIGMOID, fnone, s));
     }
-    TRYM(disp_to_depth(disp, h * w, min_depth, max_depth, baseline, depth_out, s));
+    TRYM(disp_to_depth(disp, nb * h * w, min_depth, max_depth, baseline, depth_out, s));
     return DFVO_OK;
   }
   void geometry(int* hh, int* ww) override { *hh = h; *ww = w; }
+  int batch() override { return nb; }
   size_t bytes() override { return arena.total(); }
 };
 
@@ -316,18 +328,19 @@ template <typename T>
 struct PoseImpl : public PoseNetBase {
   Arena arena;
   bool tf32 = false;
-  int h = 0, w = 0, hh = 0, ww = 0;
+  int nb = 1, h = 0, w = 0, hh = 0, ww = 0;
   float baseline = 1.f;
   Resnet18Encoder<T> enc;
   ConvLayer squeeze, pose0, pose1, pose2;
   T *dA, *dB;
-  float* out12;               // [hh][ww][16] fp32, channels 0..11 real
+  float* out12;               // [nb][hh][ww][16] fp32, channels 0..11 real
 
-  int build(const WeightStore& ws, int feed_h, int feed_w, float base) {
-    h = feed_h; w = feed_w; baseline = base;
+  int build(const WeightStore& ws, int batch, int feed_h, int feed_w, float base) {
+    nb = batch; h = feed_h; w = feed_w; baseline = base;
+    DFVO_REQUIRE(nb >= 1, DFVO_EINVAL, "PoseNet batch must be at least 1 (got %d)", nb);
     DFVO_REQUIRE(h % 32 == 0 && w % 32 == 0 && h >= 64 && w >= 64, DFVO_ESHAPE, "PoseNet feed size must be a multiple of 32 and at least 64x64 (got %dx%d)", h, w);
     enc.tf32 = tf32;
-    TRYM(enc.build_layers(arena, ws, h, w, 6));
+    TRYM(enc.build_layers(arena, ws, nb, h, w, 6));
     TRYM(plain_conv<T>(arena, tf32, ws, "net.0", 512, 0, &squeeze));
     TRYM(plain_conv<T>(arena, tf32, ws, "net.1", 256, 1, &pose0));
     TRYM(plain_conv<T>(arena, tf32, ws, "net.2", 256, 1, &pose1));
@@ -336,56 +349,58 @@ struct PoseImpl : public PoseNetBase {
                  squeeze.kh == 1 && pose2.kh == 1, DFVO_ESTATE, "PoseDecoder weights (net.0 .. net.3) have unexpected shapes");
     TRYM(enc.alloc_buffers(arena));
     hh = enc.fh[4]; ww = enc.fw[4];
-    ALLOCM(dA, T, (size_t)hh * ww * 256); ALLOCM(dB, T, (size_t)hh * ww * 256);
-    ALLOCM(out12, float, (size_t)hh * ww * 16);
+    ALLOCM(dA, T, (size_t)nb * hh * ww * 256); ALLOCM(dB, T, (size_t)nb * hh * ww * 256);
+    ALLOCM(out12, float, (size_t)nb * hh * ww * 16);
     ALLOCM(enc.chain_bars, unsigned, 4 * CHAIN_BAR_WORDS);
     return DFVO_OK;
   }
 
-  int run(const float* feed_ref, const float* feed_cur, float* pose_out, cudaStream_t s) override {
+  // feeds [ref_i, cur_i] per entry: torch.cat([ref, cur], 1) (deep_models.py:222-226) is the encoder's two 3-channel slots
+  int run_batch(const float* const* feeds, int n, float* pose_out, cudaStream_t s) override {
+    DFVO_REQUIRE(n == nb, DFVO_ESHAPE, "PoseNet: %d feed pairs given, the runner was built for a batch of %d", n, nb);
     Ten<const T> none; memset(&none, 0, sizeof(none));
-    const float* imgs[2] = {feed_ref, feed_cur};                  // torch.cat([ref, cur], 1) (deep_models.py:222-226)
-    TRYM(enc.run(imgs, s));
-    TRYM(run_conv<T>(squeeze, ctv(enc.f[4], hh, ww, 512, 512), tv(dA, hh, ww, 256, 256), ACT_RELU, none, 0, s));
-    TRYM(run_conv<T>(pose0, ctv(dA, hh, ww, 256, 256), tv(dB, hh, ww, 256, 256), ACT_RELU, none, 0, s));
-    TRYM(run_conv<T>(pose1, ctv(dB, hh, ww, 256, 256), tv(dA, hh, ww, 256, 256), ACT_RELU, none, 0, s));
+    TRYM(enc.run(feeds, s));
+    TRYM(run_conv<T>(squeeze, ctv(enc.f[4], nb, hh, ww, 512, 512), tv(dA, nb, hh, ww, 256, 256), ACT_RELU, none, 0, s));
+    TRYM(run_conv<T>(pose0, ctv(dA, nb, hh, ww, 256, 256), tv(dB, nb, hh, ww, 256, 256), ACT_RELU, none, 0, s));
+    TRYM(run_conv<T>(pose1, ctv(dB, nb, hh, ww, 256, 256), tv(dA, nb, hh, ww, 256, 256), ACT_RELU, none, 0, s));
     Ten<const float> fnone; memset(&fnone, 0, sizeof(fnone));
-    TRYM(run_conv_f32out<T>(pose2, ctv(dA, hh, ww, 256, 256), make_ten<float>(out12, 1, hh, ww, 12, 16), ACT_NONE, fnone, s));
-    return pose_head(out12, hh, ww, 16, baseline, pose_out, s);
+    TRYM(run_conv_f32out<T>(pose2, ctv(dA, nb, hh, ww, 256, 256), make_ten<float>(out12, nb, hh, ww, 12, 16), ACT_NONE, fnone, s));
+    return pose_head(out12, nb, hh, ww, 16, baseline, pose_out, s);
   }
   void geometry(int* ph, int* pw) override { *ph = h; *pw = w; }
+  int batch() override { return nb; }
   size_t bytes() override { return arena.total(); }
 };
 
-int monodepth2_create(const WeightStore& ws, int feed_h, int feed_w, int precision, float min_depth, float max_depth,
+int monodepth2_create(const WeightStore& ws, int feed_h, int feed_w, int batch, int precision, float min_depth, float max_depth,
                       float baseline, Monodepth2Base** out) {
   *out = nullptr;
   if (precision == 0 || precision == 2) {
     auto* p = new MonoImpl<float>();
     p->tf32 = precision == 2;
-    int rc = p->build(ws, feed_h, feed_w, min_depth, max_depth, baseline);
+    int rc = p->build(ws, batch, feed_h, feed_w, min_depth, max_depth, baseline);
     if (rc) { delete p; return rc; }
     *out = p;
   } else {
     auto* p = new MonoImpl<bf16>();
-    int rc = p->build(ws, feed_h, feed_w, min_depth, max_depth, baseline);
+    int rc = p->build(ws, batch, feed_h, feed_w, min_depth, max_depth, baseline);
     if (rc) { delete p; return rc; }
     *out = p;
   }
   return DFVO_OK;
 }
 
-int posenet_create(const WeightStore& ws, int feed_h, int feed_w, int precision, float baseline_multiplier, PoseNetBase** out) {
+int posenet_create(const WeightStore& ws, int feed_h, int feed_w, int batch, int precision, float baseline_multiplier, PoseNetBase** out) {
   *out = nullptr;
   if (precision == 0 || precision == 2) {
     auto* p = new PoseImpl<float>();
     p->tf32 = precision == 2;
-    int rc = p->build(ws, feed_h, feed_w, baseline_multiplier);
+    int rc = p->build(ws, batch, feed_h, feed_w, baseline_multiplier);
     if (rc) { delete p; return rc; }
     *out = p;
   } else {
     auto* p = new PoseImpl<bf16>();
-    int rc = p->build(ws, feed_h, feed_w, baseline_multiplier);
+    int rc = p->build(ws, batch, feed_h, feed_w, baseline_multiplier);
     if (rc) { delete p; return rc; }
     *out = p;
   }

@@ -142,9 +142,9 @@ int upcat_reflect(Ten<const T> lo, int up, Ten<const T> skip, Ten<T> out, cudaSt
 // sigmoid disparity -> depth (layers.py:16-25, monodepth2.py:111-138): depth = baseline / (min_disp + (max_disp-min_disp)*disp)
 int disp_to_depth(const float* disp, int n, float min_depth, float max_depth, float baseline, float* depth, cudaStream_t s);
 // PoseDecoder tail + transformation_from_parameters(invert=True) (pose_decoder.py, layers.py:28-94, monodepth2.py:102-119):
-// out12 [h][w][pitch] fp32 (channels 0..11 of net.3) -> spatial mean, x 0.01, frame 0's axis-angle / translation, 4x4 pose with
-// the translation times baseline_multiplier -> pose_out (device fp32 [4][4])
-int pose_head(const float* out12, int h, int w, int pitch, float baseline_multiplier, float* pose_out, cudaStream_t s);
+// out12 [n][h][w][pitch] fp32 (channels 0..11 of net.3) -> per entry: spatial mean, x 0.01, frame 0's axis-angle / translation,
+// 4x4 pose with the translation times baseline_multiplier -> pose_out (device fp32 [n][4][4])
+int pose_head(const float* out12, int n, int h, int w, int pitch, float baseline_multiplier, float* pose_out, cudaStream_t s);
 // cv2.resize(INTER_NEAREST) to (W,H) + preprocess_depth (dfvo.py:314-319, utils.py:89-114)
 int depth_post(const float* depth, int h, int w, int H, int W, double crop_y0, double crop_y1, double crop_x0, double crop_x1,
                float min_depth, float max_depth, float* raw_out, float* depth_out, cudaStream_t s);

@@ -105,6 +105,18 @@ int dfvo_posenet_build(dfvo_ctx* ctx, int feed_h, int feed_w, int precision, flo
  * deep_models.py:218-226); pose_out: device fp32 [4][4] row-major = inference_pose(...)[0]: transformation_from_parameters(
  * axisangle, translation, invert=True) (layers.py:28-94) with the translation times baseline_multiplier (monodepth2.py:102-119). */
 int dfvo_posenet_forward(dfvo_ctx* ctx, const float* feed_ref, const float* feed_cur, float* pose_out, void* stream);
+/* ---- batched monodepth2 / PoseNet: one forward over `batch` independent images (e.g. one frame of each of several sequences) --
+ * Every layer runs once over N = batch; entry i of the output equals what a batch-1 runner gives for entry i's feed(s), bit for
+ * bit.  dfvo_monodepth2_build / dfvo_posenet_build are these with batch = 1 (they replace any runner of the same network). */
+int dfvo_monodepth2_build_batch(dfvo_ctx* ctx, int feed_h, int feed_w, int batch, int precision, float min_depth, float max_depth,
+                                float baseline);
+/* feeds_host_array: n device pointers (host array of device pointers, as dfvo_liteflow_forward's imgs) to float [1,3,feed_h,feed_w]
+ * feeds; each entry may point anywhere.  n must equal the built batch (else DFVO_ESHAPE).  depth_out [n][feed_h][feed_w] fp32. */
+int dfvo_monodepth2_forward_batch(dfvo_ctx* ctx, const float* const* feeds_host_array, int n, float* depth_out, void* stream);
+int dfvo_posenet_build_batch(dfvo_ctx* ctx, int feed_h, int feed_w, int batch, int precision, float baseline_multiplier);
+/* feeds_host_array: 2n device pointers [ref0, cur0, ref1, cur1, ...] to float [1,3,feed_h,feed_w] feeds; n must equal the built
+ * batch (else DFVO_ESHAPE).  pose_out: device fp32 [n][4][4], entry i = dfvo_posenet_forward(ref_i, cur_i). */
+int dfvo_posenet_forward_batch(dfvo_ctx* ctx, const float* const* feeds_host_array, int n, float* pose_out, void* stream);
 /* DepthConsistency.compute (depth_consistency.py:31-163): depth_diff [H,W] = clamp(|warp - reproj| / reproj, 0, 1) where reproj is
  * the depth of depth_cur's points under T and warp = grid_sample(depth_ref, Reprojection(depth_cur, T, K, inv_K),
  * padding_mode="border", align_corners=True).  depth_cur / depth_ref: the [H,W] NEAREST-resized raw depths (not range-clamped);

@@ -1,5 +1,6 @@
 """Small pass over every kernel family of the hot path, meant to run under compute-sanitizer (memcheck / racecheck / synccheck):
-LiteFlowNet (per-layer and chained convs, fused warp+correlation), monodepth2, consistency, selection, E / H / PnP RANSAC.
+LiteFlowNet (per-layer and chained convs, fused warp+correlation), monodepth2, consistency, selection, E / H / PnP RANSAC, and a
+short two-sequence multiseq.SequenceBatch run (batched monodepth2, PoseNet and LiteFlowNet).
 No oracle here -- the parity tests do the checking; this run only has to be clean.  Usage (on a GPU):
   compute-sanitizer --tool memcheck python scripts/sanitize_run.py"""
 import os
@@ -35,6 +36,20 @@ def main():
         assert np.isfinite(fwd.numpy()).all() and np.isfinite(d).all()
         print("nets ok (chains %d)" % chain, flush=True)
     rt.lib.dfvo_set_conv_chain(0)
+    # two sequences on one GPU: batched monodepth2 / PoseNet / LiteFlowNet (S = 2), one sequence idle for a step
+    from b200 import config, multiseq
+    cfg = config.default_cfg(H, W)
+    cfg.deep_pose.enable = cfg.kp_selection.depth_consistency.enable = True
+    penc, pdec = synth.posenet_weights()
+    for overlap in (False, True):
+        b = multiseq.SequenceBatch([K, K], H, W, cfg=cfg, overlap=overlap, runtime=rt)
+        b.load_weights(synth.liteflownet_weights(), *synth.monodepth2_weights(4869, 64, 96), penc, pdec)
+        imgs = [synth.value_noise_image(H, W, 10 + i) for i in range(4)]
+        for row in ([imgs[0], imgs[1]], [imgs[2], None], [imgs[3], imgs[2]]):
+            b.step(row)
+        b.flush()
+        rt.sync()
+        print("SequenceBatch ok (overlap %d): frames tracked %s" % (overlap, [len(p) for p in b.poses]), flush=True)
     eng = tracking.Engine(376, 1241, rt)              # the synthetic correspondences / depths are KITTI-sized
     for seed, outl, still in [(31, 0.0, False), (33, 0.6, False), (34, 0.1, True)]:
         kp_ref, kp_cur, info = synthdata.correspondences(n=600, seed=seed, outlier_frac=outl, zero_motion=still)
