@@ -6,6 +6,7 @@
 #endif
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 
 #define DFVO_OK 0
 #define DFVO_EINVAL (-1)
@@ -89,6 +90,22 @@ template <typename T> DFVO_D T from_f(float v);
 template <> DFVO_D float from_f<float>(float v) { return v; }
 template <> DFVO_D __nv_bfloat16 from_f<__nv_bfloat16>(float v) {
   return __float2bfloat16_rn(v);
+}
+
+// fp32 -> tf32 grid (10-bit mantissa), round to nearest, ties away from zero: cvt.rna.tf32.f32 on the device, its bit-level
+// equivalent in the CPU test build
+DFVO_D float rna_tf32(float v) {
+#if defined(__CUDA_ARCH__)
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+  return __uint_as_float(r);
+#else
+  uint32_t u;
+  memcpy(&u, &v, 4);
+  if ((u & 0x7f800000u) != 0x7f800000u) u = (u + 0x1000u) & 0xffffe000u;
+  memcpy(&v, &u, 4);
+  return v;
+#endif
 }
 
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }

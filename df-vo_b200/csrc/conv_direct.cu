@@ -109,7 +109,8 @@ k_conv_direct(ConvDirect c, Ten<const TI> in, Ten<TO> out, Ten<const TO> res, in
       if (co >= c.Cout) continue;
       float v = acc[i][j] + (c.bias ? c.bias[co] : 0.f);
       if (has_res) v += to_f(r[co]);
-      o[co] = from_f<TO>(apply_act(v, c.act));
+      v = apply_act(v, c.act);
+      o[co] = from_f<TO>(c.round_tf32 ? rna_tf32(v) : v);
     }
   }
 }

@@ -87,6 +87,7 @@ struct Resnet18Encoder {
   int fh[5], fw[5], fc[5];
   T *pool, *tA, *tB, *tD;     // scratch at layer resolution [nb]
   unsigned* chain_bars = nullptr;     // arrival counters of the encoder's layer chain
+  LayerTap tap;
 
   int xpitch() const { return cin == 3 ? 4 : 8; }
 
@@ -166,17 +167,21 @@ struct Resnet18Encoder {
     return DFVO_OK;
   }
 
-  int basic_block(Block& B, const T* in, int ih, int iw, int ic, T* out, int oc, cudaStream_t s) {
+  // block bi of layer li + 1 (encoder.layer{li+1}.{bi})
+  int basic_block(Block& B, int li, int bi, const T* in, int ih, int iw, int ic, T* out, int oc, cudaStream_t s) {
     const int oh = ih / B.stride, ow = iw / B.stride;
     Ten<const T> none; memset(&none, 0, sizeof(none));
     TRYM(run_conv<T>(B.c1, ctv(in, nb, ih, iw, ic, ic), tv(tA, nb, oh, ow, oc, oc), ACT_RELU, none, 0, s));
+    tap(s, tv(tA, nb, oh, ow, oc, oc), "enc.layer%d.%d.conv1", li + 1, bi);
     const T* idt = in;
     if (B.has_down) {
       TRYM(run_conv<T>(B.down, ctv(in, nb, ih, iw, ic, ic), tv(tD, nb, oh, ow, oc, oc), ACT_NONE, none, 0, s));
+      tap(s, tv(tD, nb, oh, ow, oc, oc), "enc.layer%d.%d.down", li + 1, bi);
       idt = tD;
     }
     // out = relu(bn2(conv2(.)) + identity)   (torchvision BasicBlock.forward)
     TRYM(run_conv<T>(B.c2, ctv(tA, nb, oh, ow, oc, oc), tv(out, nb, oh, ow, oc, oc), ACT_RELU, ctv(idt, nb, oh, ow, oc, oc), 0, s));
+    tap(s, tv(out, nb, oh, ow, oc, oc), "enc.layer%d.%d.out", li + 1, bi);
     return DFVO_OK;
   }
 
@@ -191,6 +196,7 @@ struct Resnet18Encoder {
           Ten<T> pv; pv.p = imgpad + b * img + 3 * 8 + 3 * i; pv.N = 1; pv.H = h; pv.W = w; pv.C = 3; pv.sW = 8; pv.sH = row; pv.sN = img;
           TRYM(normalize_nchw_to_nhwc<T>(imgs[b * per + i], 1, 3, h, w, 0.45f, 0.225f, pv, s));     // borders / pad channels stay zero
         }
+      tap(s, tv(imgpad, nb, h, w + 8, 8, 8), "imgpad");
       Ten<const T> eo[2];
       for (int par = 0; par < 2; ++par) {
         Ten<const T>& v = eo[par];
@@ -202,20 +208,26 @@ struct Resnet18Encoder {
       for (int b = 0; b < nb; ++b)
         for (int i = 0; i < per; ++i)
           TRYM(normalize_nchw_to_nhwc<T>(imgs[b * per + i], 1, 3, h, w, 0.45f, 0.225f, tv(x0 + b * img + 3 * i, 1, h, w, 3, xpitch()), s));
-      ConvDirect d = {cin, 64, 7, 7, 2, 3, 3, 0, ACT_RELU, conv1.w_direct, conv1.w_pitch, conv1.bias};
+      tap(s, tv(x0, nb, h, w, xpitch(), xpitch()), "x0");
+      // tf32 mode: the stem's output reaches tf32 tensor-core layers (through the max-pool into layer1, and as decoder.7's skip),
+      // which read fp32 operands as they are; round it to the tf32 grid here like every tensor-core layer rounds its own output
+      ConvDirect d = {cin, 64, 7, 7, 2, 3, 3, 0, ACT_RELU, conv1.w_direct, conv1.w_pitch, conv1.bias, tf32 ? 1 : 0};
       TRYM((conv_direct<T, T>(d, ctv(x0, nb, h, w, cin, xpitch()), tv(f[0], nb, fh[0], fw[0], 64, 64), none, s)));
     }
+    tap(s, tv(f[0], nb, fh[0], fw[0], 64, 64), "enc.stem");
     TRYM(maxpool3x3s2<T>(ctv(f[0], nb, fh[0], fw[0], 64, 64), tv(pool, nb, fh[1], fw[1], 64, 64), s));
+    tap(s, tv(pool, nb, fh[1], fw[1], 64, 64), "enc.pool");
     const T* cur = pool;
     int ch = fh[1], cw = fw[1], cc = 64;
     {
-      // the encoder is convolutions only: consecutive stride-1 layers (c1 -> c2 of a block, and on into the next block) form chains
-      ChainScope chain(s, IsBf16m<T>::v ? chain_bars : nullptr);
+      // the encoder is convolutions only: consecutive stride-1 layers (c1 -> c2 of a block, and on into the next block) form chains.
+      // A chain defers its layers to end(), so there is none while a tap reads every layer's output right after its launch.
+      ChainScope chain(s, IsBf16m<T>::v && !tap.fn ? chain_bars : nullptr);
       for (int li = 0; li < 4; ++li) {
         const int oc = fc[li + 1];
-        TRYM(basic_block(blk[li][0], cur, ch, cw, cc, tB, oc, s));
+        TRYM(basic_block(blk[li][0], li, 0, cur, ch, cw, cc, tB, oc, s));
         ch /= blk[li][0].stride; cw /= blk[li][0].stride; cc = oc;
-        TRYM(basic_block(blk[li][1], tB, ch, cw, cc, f[li + 1], oc, s));
+        TRYM(basic_block(blk[li][1], li, 1, tB, ch, cw, cc, f[li + 1], oc, s));
         cur = f[li + 1];
       }
       TRYM(chain.end());
@@ -236,6 +248,7 @@ struct MonoImpl : public Monodepth2Base {
   T* padbuf;                  // reflection-padded conv input scratch
   T *dA, *dB;                 // decoder activations
   float* disp;
+  LayerTap tap;
 
   int build(const WeightStore& ws, int batch, int feed_h, int feed_w, float mind, float maxd, float base) {
     nb = batch; h = feed_h; w = feed_w; min_depth = mind; max_depth = maxd; baseline = base;
@@ -292,7 +305,9 @@ struct MonoImpl : public Monodepth2Base {
     for (int i = 4; i >= 0; --i) {
       // upconv(i,0): ConvBlock on x
       TRYM(upcat_reflect<T>(ctv(x, nb, xh, xw, xc, xc), 1, none, tv(padbuf, nb, xh + 2, xw + 2, xc, xc), s));
+      tap(s, tv(padbuf, nb, xh + 2, xw + 2, xc, xc), "dec.%d.pad", idx);
       TRYM(run_conv<T>(up[idx], ctv(padbuf, nb, xh + 2, xw + 2, xc, xc), tv(dA, nb, xh, xw, dec[i], dec[i]), ACT_ELU, none, 0, s));
+      tap(s, tv(dA, nb, xh, xw, dec[i], dec[i]), "dec.%d.conv", idx);
       ++idx;
       // upsample x2, concat skip, upconv(i,1)
       const int sc = i > 0 ? fc[i - 1] : 0;
@@ -300,7 +315,9 @@ struct MonoImpl : public Monodepth2Base {
       if (i > 0) skip = ctv(f[i - 1], nb, fh[i - 1], fw[i - 1], sc, sc);
       const int nh = 2 * xh, nw = 2 * xw, ncat = dec[i] + sc;
       TRYM(upcat_reflect<T>(ctv(dA, nb, xh, xw, dec[i], dec[i]), 2, skip, tv(padbuf, nb, nh + 2, nw + 2, ncat, ncat), s));
+      tap(s, tv(padbuf, nb, nh + 2, nw + 2, ncat, ncat), "dec.%d.pad", idx);
       TRYM(run_conv<T>(up[idx], ctv(padbuf, nb, nh + 2, nw + 2, ncat, ncat), tv(dB, nb, nh, nw, dec[i], dec[i]), ACT_ELU, none, 0, s));
+      tap(s, tv(dB, nb, nh, nw, dec[i], dec[i]), "dec.%d.conv", idx);
       ++idx;
       x = dB; xh = nh; xw = nw; xc = dec[i];
       // swap scratch so the next stage does not overwrite its own input
@@ -309,13 +326,17 @@ struct MonoImpl : public Monodepth2Base {
     }
     // dispconv scale 0: Conv3x3 (reflect) + sigmoid, 16 -> 1
     TRYM(upcat_reflect<T>(ctv(x, nb, xh, xw, 16, 16), 1, none, tv(padbuf, nb, xh + 2, xw + 2, 16, 16), s));
+    tap(s, tv(padbuf, nb, xh + 2, xw + 2, 16, 16), "dec.10.pad");
     {
       Ten<const float> fnone; memset(&fnone, 0, sizeof(fnone));
       TRYM(run_conv_f32out<T>(disp0, ctv(padbuf, nb, xh + 2, xw + 2, 16, 16), make_ten<float>(disp, nb, h, w, 1, 1), ACT_SIGMOID, fnone, s));
     }
+    tap(s, make_ten<float>(disp, nb, h, w, 1, 1), "disp");
     TRYM(disp_to_depth(disp, nb * h * w, min_depth, max_depth, baseline, depth_out, s));
+    tap(s, make_ten<float>(depth_out, nb, h, w, 1, 1), "depth");
     return DFVO_OK;
   }
+  void set_tap(LayerTap t) override { tap = t; enc.tap = t; }
   void geometry(int* hh, int* ww) override { *hh = h; *ww = w; }
   int batch() override { return nb; }
   size_t bytes() override { return arena.total(); }
@@ -334,6 +355,7 @@ struct PoseImpl : public PoseNetBase {
   ConvLayer squeeze, pose0, pose1, pose2;
   T *dA, *dB;
   float* out12;               // [nb][hh][ww][16] fp32, channels 0..11 real
+  LayerTap tap;
 
   int build(const WeightStore& ws, int batch, int feed_h, int feed_w, float base) {
     nb = batch; h = feed_h; w = feed_w; baseline = base;
@@ -361,12 +383,19 @@ struct PoseImpl : public PoseNetBase {
     Ten<const T> none; memset(&none, 0, sizeof(none));
     TRYM(enc.run(feeds, s));
     TRYM(run_conv<T>(squeeze, ctv(enc.f[4], nb, hh, ww, 512, 512), tv(dA, nb, hh, ww, 256, 256), ACT_RELU, none, 0, s));
+    tap(s, tv(dA, nb, hh, ww, 256, 256), "pose.net0");
     TRYM(run_conv<T>(pose0, ctv(dA, nb, hh, ww, 256, 256), tv(dB, nb, hh, ww, 256, 256), ACT_RELU, none, 0, s));
+    tap(s, tv(dB, nb, hh, ww, 256, 256), "pose.net1");
     TRYM(run_conv<T>(pose1, ctv(dB, nb, hh, ww, 256, 256), tv(dA, nb, hh, ww, 256, 256), ACT_RELU, none, 0, s));
+    tap(s, tv(dA, nb, hh, ww, 256, 256), "pose.net2");
     Ten<const float> fnone; memset(&fnone, 0, sizeof(fnone));
     TRYM(run_conv_f32out<T>(pose2, ctv(dA, nb, hh, ww, 256, 256), make_ten<float>(out12, nb, hh, ww, 12, 16), ACT_NONE, fnone, s));
-    return pose_head(out12, nb, hh, ww, 16, baseline, pose_out, s);
+    tap(s, make_ten<float>(out12, nb, hh, ww, 12, 16), "pose.out12");
+    TRYM(pose_head(out12, nb, hh, ww, 16, baseline, pose_out, s));
+    tap(s, make_ten<float>(pose_out, nb, 4, 4, 1, 1), "pose");
+    return DFVO_OK;
   }
+  void set_tap(LayerTap t) override { tap = t; enc.tap = t; }
   void geometry(int* ph, int* pw) override { *ph = h; *pw = w; }
   int batch() override { return nb; }
   size_t bytes() override { return arena.total(); }

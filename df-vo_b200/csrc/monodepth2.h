@@ -11,6 +11,9 @@ struct Monodepth2Base {
   // deep_models.py:195-201); depth_out: [n][h][w] fp32 = Monodepth2DepthNet.inference_depth (monodepth2.py:121-139) per image
   virtual int run_batch(const float* const* imgs, int n, float* depth_out, cudaStream_t s) = 0;
   int run(const float* img_nchw, float* depth_out, cudaStream_t s) { return run_batch(&img_nchw, 1, depth_out, s); }
+  // per-layer hook (net_common.h::LayerTap) of the following run_batch calls: x0 | imgpad, enc.stem, enc.pool,
+  // enc.layer{1..4}.{0,1}.{conv1,down,out}, dec.{0..10}.pad, dec.{0..9}.conv, disp, depth
+  virtual void set_tap(LayerTap t) = 0;
   virtual void geometry(int* h, int* w) = 0;
   virtual int batch() = 0;
   virtual size_t bytes() = 0;
@@ -29,6 +32,9 @@ struct PoseNetBase {
     const float* feeds[2] = {feed_ref, feed_cur};
     return run_batch(feeds, 1, pose_out, s);
   }
+  // per-layer hook of the following run_batch calls: the encoder's taps (Monodepth2Base::set_tap), pose.net0 .. pose.net2,
+  // pose.out12, pose
+  virtual void set_tap(LayerTap t) = 0;
   virtual void geometry(int* h, int* w) = 0;
   virtual int batch() = 0;
   virtual size_t bytes() = 0;

@@ -1,6 +1,8 @@
 // Host-side plumbing shared by the two network runners: weight store (reference state-dict key
 // -> fp32 host array), device arena, conv-layer packing for the two conv backends.
 #pragma once
+#include <stdarg.h>
+
 #include <map>
 #include <string>
 #include <vector>
@@ -8,6 +10,27 @@
 #include "ops.h"
 
 namespace dfvo {
+
+// Per-layer observation hook of the network runners: called right after a runner has enqueued the launch that produces a tensor,
+// with the view that launch wrote (esize: 2 = bf16, 4 = fp32 elements) and a stable name that maps to the reference state-dict
+// keys.  The callee may synchronise `s` and read the view; the next launch overwrites reused scratch.  Unset (fn == nullptr) it
+// costs one host-side pointer test per layer and changes no launch.
+struct LayerTap {
+  void (*fn)(void* user, const char* name, int esize, const void* p, int N, int H, int W, int C, long long sN, long long sH, long long sW,
+             cudaStream_t s) = nullptr;
+  void* user = nullptr;
+
+  template <typename T>
+  void operator()(cudaStream_t s, const Ten<T>& v, const char* fmt, ...) const {
+    if (!fn) return;
+    char name[64];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(name, sizeof(name), fmt, ap);
+    va_end(ap);
+    fn(user, name, (int)sizeof(T), (const void*)v.p, v.N, v.H, v.W, v.C, v.sN, v.sH, v.sW, s);
+  }
+};
 
 struct HostTensor {
   std::vector<int64_t> shape;

@@ -70,6 +70,7 @@ struct ConvDirect {
   const float* w;         // [kh*kw*Cin][Cout_pitch] fp32, k = (ky*kw+kx)*Cin + ci
   int w_pitch;            // Cout rounded up to 4
   const float* bias;      // [Cout] or nullptr
+  int round_tf32 = 0;     // fp32 output: round to the tf32 grid (cvt.rna), for a tf32 tensor-core consumer (see ConvTc::round_out_tf32)
 };
 template <typename TI, typename TO>
 int conv_direct(const ConvDirect& c, Ten<const TI> in, Ten<TO> out, Ten<const TO> residual,
