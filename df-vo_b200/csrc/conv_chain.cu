@@ -174,7 +174,7 @@ k_conv_chain(const __grid_constant__ ChainArgs P) {
         if (lane == 0 && !chain_wait(P.bar + (l - 1), gridDim.x)) *P.err = 1u;
         __syncwarp();
       }
-      TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = 0; ep.out = p.out; ep.res = p.res;
+      TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = 0; ep.vec16 = 0; ep.out = p.out; ep.res = p.res;
       switch (p.block_n) {
         case 16: chain_layer<S, 16>(p, ra, rb, ep, bias_s, wg, wq, lane, leader); break;
         case 32: chain_layer<S, 32>(p, ra, rb, ep, bias_s, wg, wq, lane, leader); break;

@@ -36,6 +36,7 @@ struct ConvHaloK {
   int Cout, Cout_pad, act, out_f32, zero_pad_to;
   int chunk;                     // channels per 128-byte operand row: 64 (bf16) or 32 (fp32 read as tf32)
   int esize, round_tf32;
+  int vec16;                     // TcEpi::vec16
   const float* bias;
   void* out; long long oN, oH, oW;
   const void* res; long long rN, rH, rW;
@@ -127,8 +128,10 @@ k_conv_halo(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CU
     for (int i = ct; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
     asm volatile("bar.sync 1, 256;" ::: "memory");
     TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = p.round_tf32; ep.out = p.out; ep.res = p.res;
+    ep.vec16 = p.vec16;
     float acc[S][BN / 2];
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x, it = 0; tile < p.ntiles; tile += gridDim.x, ++it) {
+      DFVO_HALO_STAMP(0);
       halo_tile_mma<S, BN, TF32>(acc, ra, rb, p.nsrc, p.srcC, p.chunk, p.esize, p.kh, p.kw, p.HW, wg, (ct & 127) == 0);
       int t = tile;
       const int tx = t % p.tiles_x; t /= p.tiles_x;
@@ -136,6 +139,8 @@ k_conv_halo(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CU
       const int n = t % p.N; const int nb = t / p.N;
       halo_tile_store<S, BN>(acc, ep, bias_s, nb * BN, n, tx * 8 * S, ty * HALO_TH, p.W, p.H, p.oN, p.oH, p.oW, p.rN, p.rH, p.rW, wg,
                              (ct >> 5) & 3, lane);
+      DFVO_HALO_STAMP(5);
+      DFVO_HALO_STAMP_TILE(it);
     }
   }
 }
@@ -303,6 +308,7 @@ int conv_halo(const ConvTc& c, cudaStream_t s) {
   k.zero_pad_to = c.zero_pad_to > c.Cout ? c.zero_pad_to : c.Cout;
   k.bias = c.bias; k.out = c.out; k.oN = c.oN; k.oH = c.oH; k.oW = c.oW;
   k.res = c.residual; k.rN = c.rN; k.rH = c.rH; k.rW = c.rW;
+  k.vec16 = tc_epi_vec16(c);
 
   CUtensorMap tmA[3], tmB;
   for (int i = 0; i < 3; ++i) {
@@ -340,4 +346,18 @@ int conv_halo(const ConvTc& c, cudaStream_t s) {
 }
 
 }  // namespace dfvo
+
+#ifdef DFVO_HALO_STAMPS
+// development aid (scripts/halo_phases.py): dims = {CTAs, tiles per CTA, slots per tile}; with host != NULL also copies the
+// [CTA][warpgroup][tile + 1][slot] stamp buffer of k_conv_halo out and zeroes it
+extern "C" int dfvo_halo_stamps_read(unsigned long long* host, int* dims) {
+  dims[0] = HALO_STAMP_CTAS; dims[1] = HALO_STAMP_TILES; dims[2] = HALO_STAMP_N;
+  if (!host) return 0;
+  if (cudaDeviceSynchronize() != cudaSuccess) return 1;
+  if (cudaMemcpyFromSymbol(host, dfvo::tc::g_halo_stamps, sizeof(dfvo::tc::g_halo_stamps)) != cudaSuccess) return 1;
+  void* dev = nullptr;
+  if (cudaGetSymbolAddress(&dev, dfvo::tc::g_halo_stamps) != cudaSuccess) return 1;
+  return cudaMemset(dev, 0, sizeof(dfvo::tc::g_halo_stamps)) == cudaSuccess ? 0 : 1;
+}
+#endif
 #endif  // !DFVO_HOSTSIM

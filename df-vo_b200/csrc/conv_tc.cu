@@ -50,6 +50,7 @@ struct ConvTcK {
   int block_n, stages;
   int Cout, Cout_pad, act, out_f32, zero_pad_to;
   int chunk, esize, round_tf32;   // channels per 128-byte operand row (64 bf16 / 32 tf32), operand element size
+  int vec16;                      // TcEpi::vec16
   const float* bias;
   void* out; long long oN, oH, oW;
   const void* res; long long rN, rH, rW;
@@ -141,6 +142,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     for (int i = ct; i < p.Cout_pad; i += 256) bias_s[i] = p.bias ? p.bias[i] : 0.f;
     asm volatile("bar.sync 1, 256;" ::: "memory");
     TcEpi ep; ep.Cout = p.Cout; ep.zero_pad_to = p.zero_pad_to; ep.act = p.act; ep.out_f32 = p.out_f32; ep.round_tf32 = p.round_tf32; ep.out = p.out; ep.res = p.res;
+    ep.vec16 = p.vec16;
     int stage = 0; uint32_t phase = 0;
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
@@ -176,7 +178,17 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       const int tx = t % p.tiles_x; t /= p.tiles_x;
       const int ty = t % p.tiles_y; t /= p.tiles_y;
       const int n = t % p.N; const int nb = t / p.N;
-      // accumulator pair (4 j + 2 h, +1) = tile row 64 wg + 16 wq + lane / 4 + 8 h, channels nb * BN + 8 j + 2 (lane % 4) + {0, 1}
+      // accumulator pair (4 j + 2 h, +1) = tile row 64 wg + 16 wq + lane / 4 + 8 h, channels nb * BN + 8 j + 2 (lane % 4) + {0, 1};
+      // a tile inside the image with all BN channels real stores 8-channel runs (tc_ptx.cuh::tc_store_frag16), any other pair by pair
+      if (ep.vec16 && (nb + 1) * BN <= p.Cout && (tx + 1) * p.tw <= p.W && (ty + 1) * p.th <= p.H) {
+        float (&acc1)[1][BN / 2] = reinterpret_cast<float (&)[1][BN / 2]>(acc);
+        tc_store_frag16<BN>(ep, bias_s, acc1[0], nb * BN, lane, [&](int h, long long* opix, long long* rpix) {
+          const int row = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+          const int x = tx * p.tw + (row % p.tw), y = ty * p.th + (row / p.tw);
+          *opix = n * p.oN + y * p.oH + x * p.oW; *rpix = n * p.rN + y * p.rH + x * p.rW;
+        });
+        continue;
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
@@ -247,6 +259,13 @@ void tc_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int gr
   attr->val.programmaticStreamSerializationAllowed = 1;
   cfg->attrs = attr; cfg->numAttrs = pdl ? 1 : 0;
 }
+bool tc_epi_vec16(const ConvTc& c) {
+  const long long es = c.out_f32 ? 4 : 2;
+  auto aligned = [&](const void* p, long long sN, long long sH, long long sW) {
+    return ((uintptr_t)p & 15) == 0 && (sN * es) % 16 == 0 && (sH * es) % 16 == 0 && (sW * es) % 16 == 0;
+  };
+  return aligned(c.out, c.oN, c.oH, c.oW) && (!c.residual || aligned(c.residual, c.rN, c.rH, c.rW));
+}
 int tc_num_sms() {
   if (!g_num_sms) {
     int dev = 0; cudaGetDevice(&dev);
@@ -304,6 +323,7 @@ static int build_plan(const ConvTc& c, ConvTcPlanImpl* pl) {
   k.zero_pad_to = c.zero_pad_to > c.Cout ? c.zero_pad_to : c.Cout;
   k.bias = c.bias; k.out = c.out; k.oN = c.oN; k.oH = c.oH; k.oW = c.oW;
   k.res = c.residual; k.rN = c.rN; k.rH = c.rH; k.rW = c.rW;
+  k.vec16 = tc_epi_vec16(c);
   const size_t stage_bytes = TC_A_BYTES + (size_t)k.block_n * 128;
   const size_t fixed = 1024 /*align slack*/ + 8 * 64 /*barriers*/ + 64 + (size_t)c.Cout_pad * 4 /*bias*/;
   int stages = (int)((200 * 1024 - fixed) / stage_bytes);

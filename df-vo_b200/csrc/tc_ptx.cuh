@@ -12,6 +12,7 @@ namespace dfvo {
 struct TcEpi {
   int Cout, zero_pad_to, act, out_f32;
   int round_tf32;          // fp32 output rounded to the tf32 grid (tf32 mode activations)
+  int vec16;               // output and residual base and pixel strides are 16-byte aligned: whole 8-channel runs per store
   void* out;
   const void* res;
 };
@@ -135,6 +136,102 @@ __device__ __forceinline__ void tc_store2(const TcEpi& p, const float* bias, flo
   }
 }
 
+// 4 x 4 transpose of accumulator pairs across the quad of lanes that holds one fragment row pair: on entry lane q's v[2 r + e] is
+// its pair slot r; on exit lane q's v[2 r + e] is what lane r held in slot q.  Two butterfly stages, each swapping one bit of the
+// lane index with the same bit of the slot index, with every register index a compile-time constant.  All 32 lanes must take part.
+__device__ __forceinline__ void tc_quad_transpose(float (&v)[8], int q) {
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    const bool bq = (q >> b) & 1;
+#pragma unroll
+    for (int lo = 0; lo < 4; ++lo) {
+      if (lo & (1 << b)) continue;
+      const int hi = lo | (1 << b);
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float r = __shfl_xor_sync(0xffffffffu, bq ? v[2 * lo + e] : v[2 * hi + e], 1 << b);
+        if (bq) v[2 * lo + e] = r; else v[2 * hi + e] = r;
+      }
+    }
+  }
+}
+
+// bias + optional residual + activation ACT + store of the 8 consecutive output channels c .. c + 7 of one pixel, all < Cout, with
+// 16-byte loads and stores (the caller checked TcEpi::vec16; c is a multiple of 8).  Per element the same arithmetic as tc_store2.
+template <int ACT>
+__device__ __forceinline__ void tc_store8(const TcEpi& p, const float* bias, float (&v)[8], int c, long long opix, long long rpix) {
+  uint4 rb16 = make_uint4(0u, 0u, 0u, 0u);
+  if (p.res && !p.out_f32) rb16 = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + rpix + c);
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {               // channels c + 4 k .. + 3: the fp32 residual in two 16-byte loads
+    float r[4];
+    if (p.res) {
+      if (p.out_f32) {
+        const float4 r4 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.res) + rpix + c)[k];
+        r[0] = r4.x; r[1] = r4.y; r[2] = r4.z; r[3] = r4.w;
+      } else {
+        const uint32_t w0 = k ? rb16.z : rb16.x, w1 = k ? rb16.w : rb16.y;
+        const __nv_bfloat162 b0 = *reinterpret_cast<const __nv_bfloat162*>(&w0), b1 = *reinterpret_cast<const __nv_bfloat162*>(&w1);
+        r[0] = __low2float(b0); r[1] = __high2float(b0); r[2] = __low2float(b1); r[3] = __high2float(b1);
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      float x = v[4 * k + e] + bias[c + 4 * k + e];
+      if (p.res) x += r[e];
+      v[4 * k + e] = apply_act(x, ACT);
+    }
+  }
+  if (p.out_f32) {
+    if (p.round_tf32) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[e] = tc::tc_round_tf32(v[e]);
+    }
+    float4* o = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + opix + c);
+    o[0] = make_float4(v[0], v[1], v[2], v[3]);
+    o[1] = make_float4(v[4], v[5], v[6], v[7]);
+  } else {
+    uint32_t w[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const __nv_bfloat162 b2 = __floats2bfloat162_rn(v[2 * k], v[2 * k + 1]);
+      w[k] = *reinterpret_cast<const uint32_t*>(&b2);
+    }
+    *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + opix + c) = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+// One wgmma accumulator fragment row pair (M rows r and r + 8 of a warp: pair slot 2 j + h = acc[4 j + 2 h], acc[4 j + 2 h + 1]
+// = row r + 8 h, channels 8 j + 2 (lane % 4) + {0, 1}) through tc_quad_transpose in groups of four pair slots: afterwards lane q
+// of a quad holds row r + 8 (q & 1), channels 8 (2 g + (q >> 1)) .. + 7 of group g, stored with tc_store8.  A warp store then
+// covers 16 rows x 32 contiguous bytes (bf16) instead of 8 rows x 4 B per 32-byte sector.  The warp takes this path as a whole
+// (all rows inside the image, all BN channels < Cout, vec16); pix(h) is the element offset of the lane's pixel in row r + 8 h.
+// The activation is a template parameter here: apply_act's run-time switch costs an indirect branch per element.
+template <int BN, int ACT, typename Pix>
+__device__ __forceinline__ void tc_store_frag16_act(const TcEpi& p, const float* bias, const float (&acc)[BN / 2], int cbase, int lane,
+                                                    Pix pix) {
+  const int q = lane & 3, h = q & 1;
+  long long opix, rpix;
+  pix(h, &opix, &rpix);
+#pragma unroll
+  for (int g = 0; g < BN / 16; ++g) {
+    float v[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = acc[8 * g + k];
+    tc_quad_transpose(v, q);
+    tc_store8<ACT>(p, bias, v, cbase + 8 * (2 * g + (q >> 1)), opix, rpix);
+  }
+}
+template <int BN, typename Pix>
+__device__ __forceinline__ void tc_store_frag16(const TcEpi& p, const float* bias, const float (&acc)[BN / 2], int cbase, int lane, Pix pix) {
+  switch (p.act) {
+    case ACT_LEAKY: tc_store_frag16_act<BN, ACT_LEAKY>(p, bias, acc, cbase, lane, pix); break;
+    case ACT_RELU: tc_store_frag16_act<BN, ACT_RELU>(p, bias, acc, cbase, lane, pix); break;
+    case ACT_ELU: tc_store_frag16_act<BN, ACT_ELU>(p, bias, acc, cbase, lane, pix); break;
+    case ACT_SIGMOID: tc_store_frag16_act<BN, ACT_SIGMOID>(p, bias, acc, cbase, lane, pix); break;
+    default: tc_store_frag16_act<BN, ACT_NONE>(p, bias, acc, cbase, lane, pix); break;
+  }
+}
 // An mbarrier-guarded ring of shared-memory slots as one side walks it: slot i, its full / empty barriers, the phase bit.
 struct TcRing {
   uint32_t base, slot_bytes, full0, empty0;
@@ -145,6 +242,44 @@ struct TcRing {
   __device__ __forceinline__ uint32_t empty() const { return empty0 + 8u * (uint32_t)i; }
   __device__ __forceinline__ void next() { if (++i == n) { i = 0; ph ^= 1u; } }
 };
+
+// Development aid (scripts/halo_phases.py): compiled with DFVO_HALO_STAMPS, the leader thread of each consumer warpgroup of
+// k_conv_halo records per-tile phase clocks (clock64, SM-local) into tc::g_halo_stamps; without it these macros compile to nothing
+// and the product kernels are unchanged.  Row HALO_STAMP_TILES of a (CTA, warpgroup) is the tile in progress; DFVO_HALO_STAMP_TILE
+// copies it to the row of the CTA's it-th tile.  Slots: 0 tile start, 1 first A slot full, 2 sum of A-full waits, 3 sum of
+// B-full waits, 4 last MMA retired, 5 epilogue stored.
+#ifdef DFVO_HALO_STAMPS
+#define HALO_STAMP_CTAS 288
+#define HALO_STAMP_TILES 128
+#define HALO_STAMP_N 6
+namespace tc {
+static __device__ unsigned long long g_halo_stamps[HALO_STAMP_CTAS][2][HALO_STAMP_TILES + 1][HALO_STAMP_N];
+__device__ __forceinline__ unsigned long long* halo_stamp_row(int row) {
+  return g_halo_stamps[blockIdx.x % HALO_STAMP_CTAS][(threadIdx.x >> 7) & 1][row];
+}
+}  // namespace tc
+#define DFVO_HALO_STAMP(k) \
+  do { if ((threadIdx.x & 127) == 0) tc::halo_stamp_row(HALO_STAMP_TILES)[k] = clock64(); } while (0)
+#define DFVO_HALO_TIMED(k, stmt)                                                                                  \
+  do {                                                                                                            \
+    const long long t0_ = clock64();                                                                              \
+    stmt;                                                                                                         \
+    if ((threadIdx.x & 127) == 0) tc::halo_stamp_row(HALO_STAMP_TILES)[k] += clock64() - t0_;                     \
+  } while (0)
+#define DFVO_HALO_STAMP_TILE(it)                                                                                  \
+  do {                                                                                                            \
+    if ((threadIdx.x & 127) == 0) {                                                                               \
+      unsigned long long* cur_ = tc::halo_stamp_row(HALO_STAMP_TILES);                                            \
+      if ((it) < HALO_STAMP_TILES)                                                                                \
+        for (int k_ = 0; k_ < HALO_STAMP_N; ++k_) tc::halo_stamp_row(it)[k_] = cur_[k_];                          \
+      cur_[2] = cur_[3] = 0;                                                                                      \
+    }                                                                                                             \
+  } while (0)
+#else
+#define DFVO_HALO_STAMP(k) do {} while (0)
+#define DFVO_HALO_TIMED(k, stmt) do { stmt; } while (0)
+#define DFVO_HALO_STAMP_TILE(it) do {} while (0)
+#endif
 
 // the MMAs of one tap: S sub-tiles (+8 pixels = +1024 B each) x NKS K steps (+32 B inside the 128-B swizzle atom)
 template <int S, int BN, int TF32, int NKS>
@@ -161,27 +296,31 @@ __device__ __forceinline__ void halo_tap_mma(float (&acc)[S][BN / 2], uint32_t a
 // The taps of one (source, channel chunk) of a halo tile, NKS K steps each.  NKS is a template parameter and every tap's
 // fence -> MMAs -> commit -> wait<1> is one basic block: a run-time branch between the fence and the commit makes ptxas close a
 // wgmma group inside each branch and insert an empty one at the commit (C7519 "warpgroup.arrive is injected"), so wait<1>
-// would keep only that empty group in flight and the tensor pipe would drain after every tap.
+// would keep only that empty group in flight and the tensor pipe would drain after every tap.  The chunk does not drain at its
+// end either: its last tap's group stays in flight into the next chunk.  pend_b = empty barrier of the B slot whose group may
+// still be in flight (0: none); the previous chunk's A slot (ring slot before ra.i) is released after this chunk's first
+// wait<1> unless this is the tile's first chunk (fresh == 0); the tile's last slots after its final wait<0> (halo_tile_mma).
 template <int S, int BN, int TF32, int NKS>
-__device__ __forceinline__ void halo_chunk_mma(float (&acc)[S][BN / 2], TcRing& rb, uint32_t a0, uint32_t a_sbo, int kh, int kw, int HW,
-                                               uint32_t& fresh, bool leader) {
+__device__ __forceinline__ void halo_chunk_mma(float (&acc)[S][BN / 2], const TcRing& ra, TcRing& rb, uint32_t a0, uint32_t a_sbo, int kh,
+                                               int kw, int HW, uint32_t& fresh, uint32_t& pend_b, bool leader) {
   using namespace tc;
-  int pend = -1;
+  const bool prev_a = fresh != 0u;
   for (int ky = 0; ky < kh; ++ky) {
     for (int kx = 0; kx < kw; ++kx) {
-      mbar_wait(rb.full(), rb.ph);
+      DFVO_HALO_TIMED(3, mbar_wait(rb.full(), rb.ph));
       wgmma_fence();
       halo_tap_mma<S, BN, TF32, NKS>(acc, a0 + (uint32_t)(ky * HW + kx) * 128u, rb.slot(), a_sbo, fresh);
       wgmma_commit();
       wgmma_wait<1>();
-      if (pend >= 0 && leader) mbar_arrive(rb.empty0 + 8u * (uint32_t)pend);
-      pend = rb.i;
+      if (leader) {
+        if (pend_b) mbar_arrive(pend_b);
+        if (prev_a && ky == 0 && kx == 0) mbar_arrive(ra.empty0 + 8u * (uint32_t)(ra.i ? ra.i - 1 : ra.n - 1));
+      }
+      pend_b = rb.empty();
       rb.next();
       fresh = 1u;
     }
   }
-  wgmma_wait<0>();
-  if (leader) mbar_arrive(rb.empty0 + 8u * (uint32_t)pend);
 }
 
 // MMA main loop of one tile of the halo-resident kernels (conv_halo.cu, conv_chain.cu) for one consumer warpgroup: wg 0 / 1 owns
@@ -189,46 +328,65 @@ __device__ __forceinline__ void halo_chunk_mma(float (&acc)[S][BN / 2], TcRing& 
 // halo (128 B per pixel, SWIZZLE_128B); tap (ky, kx) reads it through a descriptor whose start is shifted by (ky * HW + kx) pixels
 // and whose SBO is one halo row, so the 8-row groups of the K-major operand are the sub-tile's pixel rows.  One B slot per tap
 // (BN x 128 B of weights) is shared by the S sub-tiles and released once the MMAs of the next tap are issued and its own have
-// completed; the A slot is released at the end of its chunk.  `leader` = one thread of the warpgroup (the empty barriers count
-// one arrival per consumer warpgroup).
+// completed; an A slot likewise once the first tap of the next chunk is issued and its own last tap has completed, so the tensor
+// pipe drains only before the epilogue.  Holding the previous chunk's A slot until then cannot stall the A producer with two A
+// slots: the next chunk's slot was released when this chunk's first group retired, so the producer fills it while this chunk
+// runs, and this chunk's slot is released (at the latest by the final wait<0>) before the consumer waits on any later A slot.
+// `leader` = one thread of the warpgroup (the empty barriers count one arrival per consumer warpgroup).
 template <int S, int BN, int TF32>
 __device__ __forceinline__ void halo_tile_mma(float (&acc)[S][BN / 2], TcRing& ra, TcRing& rb, int nsrc, const int* srcC, int chunk,
                                               int esize, int kh, int kw, int HW, int wg, bool leader) {
   using namespace tc;
   const uint32_t a_sbo = (uint32_t)HW * 128u;
   uint32_t fresh = 0;                         // 0 for the first (chunk, tap) of the tile: its ks = 0 MMAs overwrite
+  uint32_t pend_b = 0u;
   for (int s = 0; s < nsrc; ++s) {
     for (int c0 = 0; c0 < srcC[s]; c0 += chunk) {
       const int rem = srcC[s] - c0;
       const int nks = ((rem >= chunk ? chunk : rem) * esize) >> 5;        // 32-byte K steps (16 bf16 / 8 tf32) with real channels
-      mbar_wait(ra.full(), ra.ph);
+      DFVO_HALO_TIMED(2, mbar_wait(ra.full(), ra.ph));
+      if (s == 0 && c0 == 0) DFVO_HALO_STAMP(1);
       const uint32_t a0 = ra.slot() + (uint32_t)wg * 8u * a_sbo;
       switch (nks) {                                                       // compile-time K steps: no wgmma in a run-time loop
-        case 4: halo_chunk_mma<S, BN, TF32, 4>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
-        case 3: halo_chunk_mma<S, BN, TF32, 3>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
-        case 2: halo_chunk_mma<S, BN, TF32, 2>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
-        default: halo_chunk_mma<S, BN, TF32, 1>(acc, rb, a0, a_sbo, kh, kw, HW, fresh, leader); break;
+        case 4: halo_chunk_mma<S, BN, TF32, 4>(acc, ra, rb, a0, a_sbo, kh, kw, HW, fresh, pend_b, leader); break;
+        case 3: halo_chunk_mma<S, BN, TF32, 3>(acc, ra, rb, a0, a_sbo, kh, kw, HW, fresh, pend_b, leader); break;
+        case 2: halo_chunk_mma<S, BN, TF32, 2>(acc, ra, rb, a0, a_sbo, kh, kw, HW, fresh, pend_b, leader); break;
+        default: halo_chunk_mma<S, BN, TF32, 1>(acc, ra, rb, a0, a_sbo, kh, kw, HW, fresh, pend_b, leader); break;
       }
-      if (leader) mbar_arrive(ra.empty());
       ra.next();
     }
+  }
+  wgmma_wait<0>();
+  DFVO_HALO_STAMP(4);
+  if (leader) {
+    mbar_arrive(pend_b);
+    mbar_arrive(ra.empty0 + 8u * (uint32_t)(ra.i ? ra.i - 1 : ra.n - 1));
   }
 }
 
 // Epilogue of one halo tile for one consumer warpgroup: the thread's accumulator pairs are pixels (x0 + 8 sub + lane / 4,
-// y0 + 8 wg + 2 warp + h), channels cbase + 8 j + 2 (lane % 4) + {0, 1}.
+// y0 + 8 wg + 2 warp + h), channels cbase + 8 j + 2 (lane % 4) + {0, 1}.  A sub-tile whose two pixel rows of this warp lie inside
+// the image, with all BN channels real and 16-byte aligned output / residual (TcEpi::vec16), is stored in 8-channel runs
+// (tc_store_frag16); anything else pair by pair (tc_store2).  The condition is uniform across the warp.
 template <int S, int BN>
 __device__ __forceinline__ void halo_tile_store(const float (&acc)[S][BN / 2], const TcEpi& ep, const float* bias_s, int cbase, int n,
                                                 int x0, int y0, int W, int H, long long oN, long long oH, long long oW, long long rN,
                                                 long long rH, long long rW, int wg, int warp_in_wg, int lane) {
+  const int yw = y0 + 8 * wg + 2 * warp_in_wg;
+  const bool vec = ep.vec16 && cbase + BN <= ep.Cout && yw + 1 < H;
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int y = y0 + 8 * wg + 2 * warp_in_wg + h;
-    if (y >= H) continue;
+  for (int sub = 0; sub < S; ++sub) {
+    const int x = x0 + 8 * sub + (lane >> 2);
+    if (vec && x0 + 8 * sub + 8 <= W) {
+      tc_store_frag16<BN>(ep, bias_s, acc[sub], cbase, lane, [&](int h, long long* opix, long long* rpix) {
+        *opix = n * oN + (yw + h) * oH + x * oW; *rpix = n * rN + (yw + h) * rH + x * rW;
+      });
+      continue;
+    }
 #pragma unroll
-    for (int sub = 0; sub < S; ++sub) {
-      const int x = x0 + 8 * sub + (lane >> 2);
-      if (x >= W) continue;
+    for (int h = 0; h < 2; ++h) {
+      const int y = yw + h;
+      if (y >= H || x >= W) continue;
       const long long opix = n * oN + y * oH + x * oW, rpix = n * rN + y * rH + x * rW;
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j)
@@ -249,6 +407,7 @@ void tc_prof_end(cudaStream_t s, const TcProf& p, double flops, const char* desc
 int tc_encode_map(void* map, const void* ptr, int rank, const unsigned long long* dims, const unsigned long long* strides_bytes,
                   const unsigned* box, int esize = 2, int swizzle_bytes = 128);   // bf16 (esize 2) or fp32 (4); swizzle 128 / 64 / 32 B; zero OOB fill
 int tc_num_sms();
+bool tc_epi_vec16(const ConvTc& c);                                  // TcEpi::vec16 of a layer: 16-byte aligned output / residual
 // launch config with the PDL attribute set unless DFVO_PDL=0 (attr must outlive the cudaLaunchKernelEx call)
 #ifndef DFVO_HOSTSIM
 void tc_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int grid, int block, size_t smem, cudaStream_t s);
