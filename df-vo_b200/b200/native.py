@@ -70,6 +70,8 @@ SIGNATURES = {
     "dfvo_conv2d": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 13 + [c_void_p]),
     "dfvo_local_bestn": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float,
                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dfvo_local_bestn_flow_ratio": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dfvo_rigid_flow_diff": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_double, c_double, c_double, c_double, c_void_p, c_void_p]),
     "dfvo_uniform_cells": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "dfvo_bestn_workspace_bytes": (c_size_t, [c_int, c_int]),

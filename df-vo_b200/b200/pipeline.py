@@ -88,6 +88,7 @@ class FramePipeline:
         self.depth_consistency = bool(self.cfg.kp_selection.depth_consistency.enable)
         if self.depth_consistency and not self.cfg.deep_pose.enable:
             raise ValueError("kp_selection.depth_consistency needs deep_pose.enable (the PoseNet gives its pose, dfvo.py:338-345)")
+        self.kp_src = self._keypoint_routing(self.cfg, self.tracking_method)
         self.K = [float(v) for v in K]
         self.H, self.W = height, width
         self.rt = runtime or rt_mod.get()
@@ -124,6 +125,37 @@ class FramePipeline:
             self.s_depths = [self.rt.new_stream() for _ in self.engs]    # monodepth2: independent of the flow network, its small
             self.s_net, self.s_depth = self.s_nets[0], self.s_depths[0]  # launches fill the SMs LiteFlowNet's coarse levels leave idle
             self.s_trk = self.rt.new_stream(high_priority=True)
+
+    @staticmethod
+    def _keypoint_routing(c, tracking_method):
+        """Which keypoint set each consumer reads (dfvo.py:165-250): {'e', 'scale', 'pnp'} -> 'kp_best' / 'kp_list'.  kp_best comes
+        from local best-N (or global best-N when only bestN.enable), kp_list from sampled_kp (keypoint_sampler.py:76-163).  A source
+        no enabled selector produces is refused here; the reference would raise KeyError on the second frame."""
+        sel = c.kp_selection
+        if sel.local_bestN.enable and sel.local_bestN.score_method not in ("flow", "flow_ratio"):
+            raise ValueError("FramePipeline implements local_bestN score_method 'flow' and 'flow_ratio', not %r"
+                             % (sel.local_bestN.score_method,))
+        produced = set()
+        if sel.local_bestN.enable or sel.bestN.get("enable", False):
+            produced.add("kp_best")
+        if sel.get("sampled_kp", {}).get("enable", False):
+            produced.add("kp_list")
+        src = dict(pnp=c.pnp_tracker.get("kp_src", "kp_best"))
+        if tracking_method == "hybrid":
+            src["e"] = c.e_tracker.get("kp_src", "kp_best")
+            s_src = c.scale_recovery.get("kp_src", "kp_best")
+            if c.scale_recovery.method == "iterative":
+                # iterative scale recovery takes kp_depth from its own rigid-flow selection, or else the E-tracker's set
+                if s_src not in ("kp_depth", src["e"]):
+                    raise ValueError("iterative scale recovery on kp_src %r needs the E-tracker's set (%r) or kp_depth" % (s_src, src["e"]))
+                s_src = src["e"]
+            src["scale"] = s_src
+        for who, name in sorted(src.items()):
+            if name not in produced:
+                raise ValueError("%s kp_src %r: no enabled keypoint selector produces it (enabled: %s)"
+                                 % ({"e": "e_tracker", "scale": "scale_recovery", "pnp": "pnp_tracker"}[who], name,
+                                    ", ".join(sorted(produced)) or "none"))
+        return src
 
     # ------------------------------------------------------------------ setup
     def load_weights(self, flow_weights, depth_enc, depth_dec, pose_enc=None, pose_dec=None):
@@ -249,10 +281,37 @@ class FramePipeline:
         ref = ref or self.ref
         fwd = cur.fwd if cur.fwd is not None else eng.flow_fwd          # (subclasses may leave the flows in the engine's buffers)
         diff = cur.diff if cur.diff is not None else eng.flow_diff
-        b = c.kp_selection.local_bestN
-        # flow validity on the fused path: the selection's one status read also carries the gate's mean flow magnitude
+        # flow validity on the fused path: the gate's mean flow magnitude of the E-tracker's set (riding on the selection's status read
+        # for local best-N)
         want_mean = self.tracking_method == "hybrid" and self.validity == "flow" and self.fused_tail
-        flow_mean = None
+        sets, good, flow_mean = self.select(cur, ref, fwd, diff, want_mean)
+        self.last = dict(good=good, n=sets[self.kp_src["e" if self.tracking_method == "hybrid" else "pnp"]][2] if good else 0, mode="const")
+        if not good:
+            return dict(pose=self.motion.copy())                          # constant motion (dfvo.py:157-161)
+        pnp_kp = sets[self.kp_src["pnp"]]
+        if self.tracking_method == "PnP":                                 # E_pose stays identity: PnP on every frame (dfvo.py:224-250)
+            kp1_buf, kp2_buf, n = pnp_kp
+            self.last["mode"] = "PnP"
+            if self.fused_tail and n <= eng.TAIL_MAX_N:
+                return dict(pnp=self.pnp_fused_launch(kp1_buf, kp2_buf, n, ref))
+            return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
+        kp1_buf, kp2_buf, n = sets[self.kp_src["e"]]
+        iterative = c.scale_recovery.method == "iterative"
+        same_scale = self.kp_src["scale"] == self.kp_src["e"]
+        if not iterative and same_scale and 10 < n <= eng.TAIL_MAX_N and self.fused_tail:
+            return self.track_fused_launch(cur, ref, kp1_buf, kp2_buf, n, flow_mean, pnp_kp)
+        return dict(pose=self.track_stepwise(cur, ref, kp1_buf, kp2_buf, n, None if same_scale else sets[self.kp_src["scale"]], pnp_kp))
+
+    def select(self, cur, ref, fwd, diff, want_mean=False):
+        """KeypointSampler.kp_selection (keypoint_sampler.py:76-143, dfvo.py:140-150) on the device: the keypoint sets the
+        configuration enables -> ({'kp_best' / 'kp_list': (kp1, kp2, n)}, good_kp_found, flow mean).  good_kp_found comes from local
+        best-N only (best-N and sampled_kp never fail); when it is False no other set is gathered.  want_mean: also the mean flow
+        magnitude of the E-tracker's set (None otherwise)."""
+        c, eng, K = self.cfg, self.eng, self.K
+        sel = c.kp_selection
+        b = sel.local_bestN
+        e_src = self.kp_src.get("e")
+        sets, good, flow_mean = {}, True, None
         if b.enable:
             dd, dthre = None, 0.05
             if self.depth_consistency:                                    # DepthConsistency.compute (dfvo.py:142-143)
@@ -261,26 +320,24 @@ class FramePipeline:
                 dd = eng.depth_consistency(cur.raw_depth, ref.raw_depth, cur.deep_pose, Km, np.linalg.inv(Km),
                                            out=self._buf("ddiff", (self.H, self.W), np.float32))
                 dthre = float(c.kp_selection.depth_consistency.thre)
-            sel = eng.select_local_bestn(diff, fwd, b.num_row, b.num_col, b.num_bestN, b.thre, depth_diff_buf=dd, depth_thre=dthre,
-                                         with_flow_mean=want_mean)
-            good, n, kp1_buf, kp2_buf = sel[:4]
-            flow_mean = sel[4] if want_mean else None
-        else:
-            good, n, kp1_buf, kp2_buf = eng.select_bestn(diff, fwd, c.kp_selection.bestN.num_bestN)
-            if want_mean:
+            mean_here = want_mean and e_src == "kp_best"
+            r = eng.select_local_bestn(diff, fwd, b.num_row, b.num_col, b.num_bestN, b.thre, depth_diff_buf=dd, depth_thre=dthre,
+                                       with_flow_mean=mean_here, score_method=b.score_method)
+            good = r[0]
+            sets["kp_best"] = (r[2], r[3], r[1])
+            if mean_here:
+                flow_mean = r[4]
+        elif sel.bestN.get("enable", False):
+            _, n, kp1_buf, kp2_buf = eng.select_bestn(diff, fwd, sel.bestN.num_bestN)
+            sets["kp_best"] = (kp1_buf, kp2_buf, n)
+            if want_mean and e_src == "kp_best":
                 flow_mean = eng.flow_mean(kp1_buf, kp2_buf, n)
-        self.last = dict(good=good, n=n, mode="const")
-        if not good:
-            return dict(pose=self.motion.copy())                          # constant motion (dfvo.py:157-161)
-        if self.tracking_method == "PnP":                                 # E_pose stays identity: PnP on every frame (dfvo.py:224-250)
-            self.last["mode"] = "PnP"
-            if self.fused_tail and n <= eng.TAIL_MAX_N:
-                return dict(pnp=self.pnp_fused_launch(kp1_buf, kp2_buf, n, ref))
-            return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
-        iterative = c.scale_recovery.method == "iterative"
-        if not iterative and 10 < n <= eng.TAIL_MAX_N and self.fused_tail:
-            return self.track_fused_launch(cur, ref, kp1_buf, kp2_buf, n, flow_mean)
-        return dict(pose=self.track_stepwise(cur, ref, kp1_buf, kp2_buf, n))
+        sk = sel.get("sampled_kp", {})
+        if good and sk.get("enable", False):
+            sets["kp_list"] = eng.sampled_keypoints(fwd, c.crop.flow_crop, sk.num_kp)
+            if want_mean and e_src == "kp_list":
+                flow_mean = eng.flow_mean(sets["kp_list"][0], sets["kp_list"][1], sets["kp_list"][2])
+        return sets, good, flow_mean
 
     def track_finish(self, tok):
         """Second half of `track`: the relative pose cur -> ref (4x4)."""
@@ -290,13 +347,19 @@ class FramePipeline:
             return self.pnp_fused_finish(tok["pnp"])
         return self.track_fused_finish(tok)
 
-    def track_stepwise(self, cur, ref, kp1_buf, kp2_buf, n):
+    def track_stepwise(self, cur, ref, kp1_buf, kp2_buf, n, scale_kp=None, pnp_kp=None):
         """The E branch with the host in the loop after every stage (iterative scale recovery, tiny / huge keypoint sets,
-        DFVO_FUSED_TAIL=0)."""
+        DFVO_FUSED_TAIL=0, or a scale recovery on another keypoint set than the E-tracker's).  scale_kp / pnp_kp: (kp1, kp2, n) of
+        the scale recovery's / PnP tracker's set when it is not the E-tracker's (scale_recovery.kp_src, pnp_tracker.kp_src)."""
         c, eng, K = self.cfg, self.eng, self.K
         iterative = c.scale_recovery.method == "iterative"
         kp_ref = kp1_buf.numpy()[:n]
         kp_cur = kp2_buf.numpy()[:n]
+        if scale_kp is not None:
+            s1, s2, sn = scale_kp
+            s_ref, s_cur, s_buf = s1.numpy()[:sn], s2.numpy()[:sn], s2
+        else:
+            s_ref, s_cur, s_buf, sn = kp_ref, kp_cur, kp2_buf, n
         # ---- E-tracker (dfvo.py:165-193).  The homography vote runs on a host worker thread; the pose-dependent device
         # work of the scale recovery (triangulation, depth gather) is issued before the vote is joined.
         r = tracking.compute_pose_2d2d(eng, kp_ref, kp_cur, K, repeat=c.e_tracker.ransac.repeat,
@@ -307,7 +370,7 @@ class FramePipeline:
         if np.linalg.norm(r["t"]) != 0 and not iterative:
             E_spec = np.eye(4)
             E_spec[:3, :3], E_spec[:3, 3:] = r["R"], r["t"]
-            prep = self.scale_prepare(kp_ref, kp_cur, kp2_buf, np.linalg.inv(E_spec), cur.depth, n)
+            prep = self.scale_prepare(s_ref, s_cur, s_buf, np.linalg.inv(E_spec), cur.depth, sn)
         tracking.resolve_validity(r)
         E_pose = np.eye(4)
         E_pose[:3, :3], E_pose[:3, 3:] = r["R"], r["t"]
@@ -322,11 +385,20 @@ class FramePipeline:
         self.last["scale"] = scale
         # ---- PnP fallback (dfvo.py:225-250)
         if np.linalg.norm(E_pose[:3, 3]) == 0 or scale == -1:
-            hybrid = self.pnp(kp_ref, kp_cur, kp1_buf, n, ref)
+            if pnp_kp is None or pnp_kp[0] is kp1_buf:
+                hybrid = self.pnp(kp_ref, kp_cur, kp1_buf, n, ref)
+            else:
+                p1, p2, pn = pnp_kp
+                hybrid = self.pnp(p1.numpy()[:pn], p2.numpy()[:pn], p1, pn, ref)
             self.last["mode"] = "PnP"
         return hybrid
 
-    def track_fused_launch(self, cur, ref, kp1_buf, kp2_buf, n, flow_mean=None):
+    def _pnp_on(self, pnp_kp, ref):
+        """PnP tracker (the fallback) on the set (kp1, kp2, n) of pnp_tracker.kp_src."""
+        p1, p2, pn = pnp_kp
+        return self.pnp(p1.numpy()[:pn], p2.numpy()[:pn], p1, pn, ref)
+
+    def track_fused_launch(self, cur, ref, kp1_buf, kp2_buf, n, flow_mean=None, pnp_kp=None):
         """The E branch of `track` with the device-side tail (tracking.Engine.essential_tail): after the keypoint count is known the
         host draws the five shuffles, enqueues the homography model, the essential-matrix repeats and the fused tail, and reads ONE
         packed result -- instead of eleven small reads with host arithmetic in between (keypoints, RANSAC info, GRIC, mask, pose,
@@ -334,19 +406,20 @@ class FramePipeline:
         keypoints are fetched only when the PnP fallback needs them.
         flow_mean (e_tracker.validity.method 'flow', E_tracker.py:182-186,249-257): the mean flow magnitude the selection read
         returned.  A closed gate draws no shuffle and leaves E_pose at identity, so the PnP fallback runs; otherwise the tail uses
-        the flow-mode validity and no homography is launched."""
+        the flow-mode validity and no homography is launched.  pnp_kp: (kp1, kp2, n) of the PnP fallback's set (default: this one)."""
         c, eng, K = self.cfg, self.eng, self.K
+        pnp_kp = pnp_kp or (kp1_buf, kp2_buf, n)
         if flow_mean is not None:
             self.last["flow_mean"] = flow_mean
             if not flow_mean > c.e_tracker.validity.thre:
                 self.last.update(valid=False, inliers=np.ones(n, bool), mode="PnP", scale=None)
-                return dict(pose=self.pnp(kp1_buf.numpy()[:n], kp2_buf.numpy()[:n], kp1_buf, n, ref))
+                return dict(pose=self._pnp_on(pnp_kp, ref))
         rs = c.scale_recovery.ransac
         perms = tracking.shuffles(self.rng, n, c.e_tracker.ransac.repeat)
         h = eng.homography_launch(kp2_buf, kp1_buf, n) if flow_mean is None else None
         w = eng.essential_launch(kp2_buf, kp1_buf, n, perms, K, threshold=c.e_tracker.ransac.reproj_thre)
         tail = eng.essential_tail_launch(w, h, kp2_buf, kp1_buf, n, K, cur.depth, self.rng, rs.min_samples, rs.max_trials, rs.stop_prob, rs.thre)
-        return dict(tail=tail, w=w, ref=ref, kp1_buf=kp1_buf, kp2_buf=kp2_buf, n=n, last=self.last)
+        return dict(tail=tail, w=w, ref=ref, kp1_buf=kp1_buf, kp2_buf=kp2_buf, n=n, last=self.last, pnp_kp=pnp_kp)
 
     def pnp_fused_launch(self, kp1_buf, kp2_buf, n, ref=None):
         """PnP tracker on the device keypoints (Engine.pnp_tail_launch): filter + unprojection, one read of the filtered count, the
@@ -377,8 +450,7 @@ class FramePipeline:
                 hybrid[:3, 3] = t[:, 0] * scale
         self.last["scale"] = scale
         if np.linalg.norm(t) == 0 or scale == -1:                    # PnP fallback (dfvo.py:225-250)
-            kp_ref, kp_cur = kp1_buf.numpy()[:n], kp2_buf.numpy()[:n]
-            hybrid = self.pnp(kp_ref, kp_cur, kp1_buf, n, ref)
+            hybrid = self._pnp_on(tok.get("pnp_kp") or (kp1_buf, kp2_buf, n), ref)
             self.last["mode"] = "PnP"
         return hybrid
 

@@ -71,7 +71,7 @@ class Engine:
         self._subsets = collections.OrderedDict()    # (N, iters) -> device table of OpenCV's subset stream; LRU-bounded
         self._subsets_cap = 256
         self._ess_ws, self._h_ws, self._pnp_ws = {}, {}, {}
-        self._sel, self._bsel, self._rf = {}, {}, {}
+        self._sel, self._bsel, self._rf, self._samp = {}, {}, {}, {}
         self.kp_capacity = 2048
 
     # ------------------------------------------------------------------ networks
@@ -194,11 +194,15 @@ class Engine:
 
     # ------------------------------------------------------------------ selection
     def select_local_bestn(self, diff_buf, flow_fwd_buf, rows, cols, num_bestN, thre, depth_diff_buf=None, depth_thre=0.05,
-                           with_flow_mean=False):
+                           with_flow_mean=False, score_method="flow"):
         """local_bestN (kp_selection.py:74-200) + keypoint gather.  Returns (good, n, kp1, kp2, mask-less)
         with kp buffers float64 [num_bestN, 2] (first n rows valid).  One small D2H (status).
         with_flow_mean: the same single read also carries the mean flow magnitude of the selection (the E-tracker's 'flow'
-        validity gate, dfvo_flow_mean), appended as a fifth element."""
+        validity gate, dfvo_flow_mean), appended as a fifth element.
+        score_method 'flow_ratio' (kp_selection.py:135-160): the cells select on flow_diff / |flow| (dfvo_local_bestn_flow_ratio);
+        that ratio map, the reference's fb_flow_mask, stays on the device as :attr:`flow_ratio_map` [H,W] until the next call."""
+        if score_method not in ("flow", "flow_ratio"):
+            raise ValueError("local_bestN score_method %r: 'flow' and 'flow_ratio' are implemented" % (score_method,))
         quota = num_bestN // (rows * cols)
         key = (rows, cols, quota)
         if key not in self._sel:
@@ -207,8 +211,16 @@ class Engine:
                                   kp2=self.rt.empty((rows * cols * quota, 2), np.float64), n=self.rt.empty((1,), np.int32))
         s = self._sel[key]
         st = self.rt.stream_ptr()
-        self.lib.check(self.lib.dfvo_local_bestn(diff_buf.ptr, depth_diff_buf.ptr if depth_diff_buf else None, self.H, self.W,
-                                                 rows, cols, num_bestN, thre, depth_thre, s["idx"].ptr, s["cc"].ptr, s["st"].ptr, st))
+        dd = depth_diff_buf.ptr if depth_diff_buf else None
+        if score_method == "flow_ratio":
+            if getattr(self, "flow_ratio_map", None) is None:
+                self.flow_ratio_map = self.rt.empty((self.H, self.W), np.float32)
+            self.lib.check(self.lib.dfvo_local_bestn_flow_ratio(diff_buf.ptr, flow_fwd_buf.ptr, dd, self.H, self.W, rows, cols, num_bestN,
+                                                                thre, depth_thre, self.flow_ratio_map.ptr, s["idx"].ptr, s["cc"].ptr,
+                                                                s["st"].ptr, st))
+        else:
+            self.lib.check(self.lib.dfvo_local_bestn(diff_buf.ptr, dd, self.H, self.W, rows, cols, num_bestN, thre, depth_thre,
+                                                     s["idx"].ptr, s["cc"].ptr, s["st"].ptr, st))
         self.lib.check(self.lib.dfvo_gather_keypoints(s["idx"].ptr, s["cc"].ptr, rows * cols, quota, flow_fwd_buf.ptr, self.H,
                                                       self.W, s["kp1"].ptr, s["kp2"].ptr, s["n"].ptr, st))
         if with_flow_mean:                                        # the mean flow magnitude travels with the status (one read)
@@ -219,6 +231,33 @@ class Engine:
             return bool(o[0]), int(o[1]), s["kp1"], s["kp2"], float(o[2])
         status = s["st"].numpy()
         return bool(status[0]), int(status[1]), s["kp1"], s["kp2"]
+
+    def sampled_keypoints(self, flow_fwd_buf, crop, num_kp, kp_list=None):
+        """sampled_kp (kp_selection.py:327-378): kp1 = (x, y) of the uniform list of generate_kp_samples (keypoint_sampler.py:52-74)
+        inside the flow crop, kp2 = kp1 + flow, float64 [num_kp, 2] device buffers.  The list is a constant of (H, W, crop, num_kp):
+        it is computed once on the host with the reference's own np.linspace, turned into full-image linear indices and uploaded;
+        each call is then one dfvo_gather_keypoints, with no read.  Returns (kp1, kp2, num_kp); the buffers are reused by the
+        next call with the same (crop, num_kp).  kp_list: the caller's own index list into the cropped grid (KeypointSampler.kps),
+        used instead of the computed one."""
+        (cy0, cy1), (cx0, cx1) = crop
+        y0, y1 = int(cy0 * self.H), int(cy1 * self.H)
+        x0, x1 = int(cx0 * self.W), int(cx1 * self.W)
+        if kp_list is not None:
+            kp_list = np.asarray(kp_list, np.int64).reshape(-1)
+            num_kp = kp_list.shape[0]
+        num_kp = int(num_kp)
+        key = (y0, y1, x0, x1, num_kp, None if kp_list is None else kp_list.tobytes())
+        c = self._samp
+        if key not in c:
+            if kp_list is None:
+                kp_list = np.linspace(0, (x1 - x0) * (y1 - y0) - 1, num_kp, dtype=int)
+            cw = x1 - x0
+            lin = ((y0 + kp_list // cw) * self.W + (x0 + kp_list % cw)).astype(np.int32)
+            c[key] = dict(idx=self.rt.from_host(lin), kp1=self.rt.empty((num_kp, 2), np.float64), kp2=self.rt.empty((num_kp, 2), np.float64))
+        s = c[key]
+        self.lib.check(self.lib.dfvo_gather_keypoints(s["idx"].ptr, None, 1, num_kp, flow_fwd_buf.ptr, self.H, self.W, s["kp1"].ptr,
+                                                      s["kp2"].ptr, None, self.rt.stream_ptr()))
+        return s["kp1"], s["kp2"], num_kp
 
     def flow_mean(self, kp_ref_buf, kp_cur_buf, n):
         """np.mean(np.linalg.norm(kp_ref - kp_cur, axis=1)) of n device keypoint pairs, bit-equal to NumPy (E_tracker.py:184)."""

@@ -442,8 +442,21 @@ int dfvo_local_bestn(const float* flow_diff, const float* depth_diff, int H, int
   DFVO_REQUIRE(flow_diff && idx_out && cell_counts && status && H > 0 && W > 0 && rows > 0 && cols > 0, DFVO_EINVAL, "dfvo_local_bestn args");
   int quota = num_bestN / (rows * cols);
   DFVO_REQUIRE(quota > 0, DFVO_EINVAL, "dfvo_local_bestn: num_bestN < rows*cols");
-  return local_bestn(flow_diff, depth_diff, H, W, rows, cols, quota, thre, depth_thre, num_bestN, idx_out, cell_counts, status,
+  return local_bestn(flow_diff, flow_diff, depth_diff, H, W, rows, cols, quota, thre, depth_thre, num_bestN, idx_out, cell_counts, status,
                      (cudaStream_t)stream);
+  API_END
+}
+
+int dfvo_local_bestn_flow_ratio(const float* flow_diff, const float* flow_fwd, const float* depth_diff, int H, int W, int rows, int cols,
+                                int num_bestN, float thre, float depth_thre, float* ratio_out, int32_t* idx_out, int32_t* cell_counts,
+                                int32_t* status, void* stream) {
+  API_BEGIN
+  DFVO_REQUIRE(flow_diff && flow_fwd && ratio_out && idx_out && cell_counts && status && H > 0 && W > 0 && rows > 0 && cols > 0,
+               DFVO_EINVAL, "dfvo_local_bestn_flow_ratio args");
+  const int quota = num_bestN / (rows * cols);
+  DFVO_REQUIRE(quota > 0, DFVO_EINVAL, "dfvo_local_bestn_flow_ratio: num_bestN < rows*cols");
+  return local_bestn_flow_ratio(flow_diff, flow_fwd, depth_diff, H, W, rows, cols, quota, thre, depth_thre, num_bestN, ratio_out, idx_out,
+                                cell_counts, status, (cudaStream_t)stream);
   API_END
 }
 

@@ -156,9 +156,14 @@ int lanczos_resize_u8(const uint8_t* img, int H, int W, const int32_t* bounds_h,
                       uint8_t* out_u8, float* out_nchw, cudaStream_t s);
 
 // ---- keypoint selection (select.cu) -------------------------------------------------------------
-int local_bestn(const float* diff, const float* depth_diff, int H, int W, int rows, int cols, int n_best,
+// count_map: the map counted for status[2] (nullptr: already counted by the caller); score: the map the cells select on
+int local_bestn(const float* count_map, const float* score, const float* depth_diff, int H, int W, int rows, int cols, int n_best,
                 float thre, float depth_thre, int N_total, int32_t* idx_out, int32_t* cell_counts,
                 int32_t* status, cudaStream_t s);
+// score_method 'flow_ratio': ratio_out = flow_diff / |flow_fwd| [H,W], then local_bestn on it (status[2] counts the raw flow_diff)
+int local_bestn_flow_ratio(const float* flow_diff, const float* flow_fwd, const float* depth_diff, int H, int W, int rows, int cols,
+                           int n_best, float thre, float depth_thre, int N_total, float* ratio_out, int32_t* idx_out, int32_t* cell_counts,
+                           int32_t* status, cudaStream_t s);
 int bestn(const float* diff, int H, int W, int N, int32_t* idx_out, void* workspace, size_t ws_bytes,
           cudaStream_t s);
 size_t bestn_workspace_bytes(int H, int W);

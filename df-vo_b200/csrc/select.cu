@@ -10,6 +10,9 @@
 // unsigned bit pattern is order-preserving) + ordered compaction.  One 256-thread block per cell.
 //
 // bestN: the same radix select over the whole map (kp_selection.py:33-71).
+//
+// score_method 'flow_ratio' (kp_selection.py:135-160,192-199): the same selection on the ratio map flow_diff / |flow|, which
+// k_flow_ratio writes while it counts the raw flow_diff < thre of the "case 1" early-out.
 #include "ops.h"
 
 namespace dfvo {
@@ -248,18 +251,53 @@ __global__ void k_local_bestn_status(const int32_t* __restrict__ cell_counts, in
   status[0] = good; status[1] = good ? sel : 0; status[3] = nonempty;
 }
 
-int local_bestn(const float* diff, const float* depth_diff, int H, int W, int rows, int cols, int n_best, float thre,
-                float depth_thre, int N_total, int32_t* idx_out, int32_t* cell_counts, int32_t* status, cudaStream_t s) {
+// local_bestN's score map for score_method 'flow_ratio' (kp_selection.py:146-149,193-197): ratio = flow_diff / ||flow||, the norm
+// as NumPy computes np.linalg.norm(axis=3) in float32 -- sqrt(fx*fx + fy*fy) with every operation rounded on its own (no FMA) --
+// so the map is bit-equal to the reference's fb_flow_mask; 0/0 gives NaN and x/0 inf, and neither passes `< thre`.  The same pass
+// counts the RAW flow_diff < thre into *count: the "case 1" early-out (kp_selection.py:121-125) tests flow_diff, not the ratio.
+__global__ void k_flow_ratio(const float* __restrict__ diff, const float* __restrict__ flow, int n, float thre, float* __restrict__ ratio,
+                             int32_t* __restrict__ count) {
+  __shared__ int scratch[SEL_THREADS];
+  int c = 0;
+  for (int i = blockIdx.x * SEL_THREADS + threadIdx.x; i < n; i += gridDim.x * SEL_THREADS) {
+    const float d = diff[i], fx = flow[i], fy = flow[(size_t)n + i];
+    const float nrm = __fsqrt_rn(__fadd_rn(__fmul_rn(fx, fx), __fmul_rn(fy, fy)));
+    ratio[i] = __fdiv_rn(d, nrm);
+    c += d < thre ? 1 : 0;
+  }
+  int total;
+  block_exclusive_scan(c, scratch, &total);
+  if (threadIdx.x == 0 && total) atomicAdd(count, total);
+}
+
+// count_map: the map whose `< thre` count is status[2] (case 1); nullptr when the caller has already zeroed the status and
+// counted into status[2] itself.  score: the map the cells select on.
+int local_bestn(const float* count_map, const float* score, const float* depth_diff, int H, int W, int rows, int cols, int n_best,
+                float thre, float depth_thre, int N_total, int32_t* idx_out, int32_t* cell_counts, int32_t* status, cudaStream_t s) {
   DFVO_REQUIRE(rows > 0 && cols > 0 && n_best > 0 && rows * cols <= 65535, DFVO_EINVAL, "local_bestn args");
-  DFVO_CUDA(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), s));
-  DFVO_LAUNCH(k_count_below, dim3(132), dim3(SEL_THREADS), 0, s, diff, H * W, thre, status + 2);
-  DFVO_CHECK_LAUNCH();
-  DFVO_LAUNCH(k_local_bestn, dim3(rows * cols), dim3(SEL_THREADS), 0, s, diff, depth_diff, H, W, rows, cols, n_best, thre,
+  if (count_map) {
+    DFVO_CUDA(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), s));
+    DFVO_LAUNCH(k_count_below, dim3(132), dim3(SEL_THREADS), 0, s, count_map, H * W, thre, status + 2);
+    DFVO_CHECK_LAUNCH();
+  }
+  DFVO_LAUNCH(k_local_bestn, dim3(rows * cols), dim3(SEL_THREADS), 0, s, score, depth_diff, H, W, rows, cols, n_best, thre,
               depth_thre, idx_out, cell_counts);
   DFVO_CHECK_LAUNCH();
   DFVO_LAUNCH(k_local_bestn_status, dim3(1), dim3(32), 0, s, cell_counts, rows * cols, N_total, status);
   DFVO_CHECK_LAUNCH();
   return DFVO_OK;
+}
+
+int local_bestn_flow_ratio(const float* flow_diff, const float* flow_fwd, const float* depth_diff, int H, int W, int rows, int cols,
+                           int n_best, float thre, float depth_thre, int N_total, float* ratio_out, int32_t* idx_out, int32_t* cell_counts,
+                           int32_t* status, cudaStream_t s) {
+  DFVO_REQUIRE(rows > 0 && cols > 0 && n_best > 0 && rows * cols <= 65535, DFVO_EINVAL, "local_bestn_flow_ratio args");
+  const int n = H * W;
+  DFVO_CUDA(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), s));
+  const int blocks = cdiv(n, SEL_THREADS) < 1056 ? cdiv(n, SEL_THREADS) : 1056;
+  DFVO_LAUNCH(k_flow_ratio, dim3(blocks), dim3(SEL_THREADS), 0, s, flow_diff, flow_fwd, n, thre, ratio_out, status + 2);
+  DFVO_CHECK_LAUNCH();
+  return local_bestn(nullptr, ratio_out, depth_diff, H, W, rows, cols, n_best, thre, depth_thre, N_total, idx_out, cell_counts, status, s);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -14,7 +14,7 @@ def _dev(x, dtype):
     return runtime.get().from_host(np.ascontiguousarray(x, dtype))
 
 
-def _finish(outputs, good, n, kp1, kp2, ref_data):
+def _finish(outputs, good, n, kp1, kp2, ref_data, mask=None):
     if not good:
         print("Cannot find enough good keypoints!")
         outputs["good_kp_found"] = False
@@ -24,23 +24,29 @@ def _finish(outputs, good, n, kp1, kp2, ref_data):
     outputs["kp2_best"] = kp2.numpy()[:n][None]
     fd = ref_data["flow_diff"]
     h, w = fd.shape[0], fd.shape[1]
-    outputs["fb_flow_mask"] = tracking.DevArray(fd.dev, (h, w)) if isinstance(fd, tracking.DevArray) else np.asarray(fd)[:, :, 0]
+    if mask is not None:
+        outputs["fb_flow_mask"] = tracking.DevArray(mask, (h, w))
+    else:
+        outputs["fb_flow_mask"] = tracking.DevArray(fd.dev, (h, w)) if isinstance(fd, tracking.DevArray) else np.asarray(fd)[:, :, 0]
     return outputs
 
 
 def local_bestN(kp1, kp2, ref_data, cfg, outputs):
-    """kp_selection.py:74-200 (score_method 'flow'); ``kp1``/``kp2`` (the dense grids of the reference) are
-    accepted for signature compatibility and ignored -- the kernel derives them from the flow."""
+    """kp_selection.py:74-200 (score_method 'flow' or 'flow_ratio'); ``kp1``/``kp2`` (the dense grids of the reference) are
+    accepted for signature compatibility and ignored -- the kernel derives them from the flow.  With 'flow_ratio' the
+    ``fb_flow_mask`` output is the device ratio map flow_diff / |flow| (the engine's buffer, rewritten by its next selection)."""
     b = cfg.kp_selection.local_bestN
-    assert b.score_method == "flow", "dfvo_b200 implements local_bestN score_method 'flow' (the default)"
+    assert b.score_method in ("flow", "flow_ratio"), "dfvo_b200 implements local_bestN score_method 'flow' and 'flow_ratio'"
     eng = tracking.default_engine()
     fd = ref_data["flow_diff"]
     assert (fd.shape[0], fd.shape[1]) == (eng.H, eng.W)
     dc = cfg.kp_selection.depth_consistency
     dd = _dev(ref_data["depth_diff"], np.float32) if dc.enable else None          # kp_selection.py:118-148
     good, n, k1, k2 = eng.select_local_bestn(_dev(fd, np.float32), _dev(ref_data["flow"], np.float32), b.num_row, b.num_col,
-                                             b.num_bestN, b.thre, dd, float(dc.thre) if dc.enable else 0.05)
-    return _finish(outputs, good, n, k1, k2, ref_data)
+                                             b.num_bestN, b.thre, dd, float(dc.thre) if dc.enable else 0.05,
+                                             score_method=b.score_method)
+    mask = eng.flow_ratio_map if b.score_method == "flow_ratio" else None
+    return _finish(outputs, good, n, k1, k2, ref_data, mask)
 
 
 def bestN_flow_kp(kp1, kp2, ref_data, cfg, outputs):
@@ -52,16 +58,11 @@ def bestN_flow_kp(kp1, kp2, ref_data, cfg, outputs):
 
 
 def sampled_kp(kp1, kp2, ref_data, kp_list, cfg, outputs):
-    """kp_selection.py:327-378: uniform sub-sampling of the (cropped) dense grid -- a pure gather."""
-    flow = np.asarray(ref_data["flow"])
-    _, h, w = flow.shape
-    y0, y1 = [int(v * h) for v in cfg.crop.flow_crop[0]]
-    x0, x1 = [int(v * w) for v in cfg.crop.flow_crop[1]]
-    ys, xs = np.meshgrid(np.arange(y0, y1), np.arange(x0, x1), indexing="ij")
-    ys, xs = ys.reshape(-1)[kp_list], xs.reshape(-1)[kp_list]
-    k1 = np.stack([xs, ys], 1).astype(np.float64)
-    k2 = k1 + np.stack([flow[0, ys, xs], flow[1, ys, xs]], 1).astype(np.float64)
-    outputs["kp1_list"], outputs["kp2_list"] = k1[None], k2[None]
+    """kp_selection.py:327-378: the (cropped) dense grid at the indices ``kp_list`` -- a gather on the device-resident flow
+    (Engine.sampled_keypoints); only the float64 [1, N, 2] keypoints come back to the host."""
+    eng = tracking.default_engine()
+    k1, k2, n = eng.sampled_keypoints(_dev(ref_data["flow"], np.float32), cfg.crop.flow_crop, len(kp_list), kp_list=kp_list)
+    outputs["kp1_list"], outputs["kp2_list"] = k1.numpy()[:n][None], k2.numpy()[:n][None]
     return outputs
 
 

@@ -175,12 +175,22 @@ int dfvo_conv2d(const float* x, const float* w_host, const float* bias_host, flo
 int dfvo_local_bestn(const float* flow_diff, const float* depth_diff, int H, int W, int rows, int cols,
                      int num_bestN, float thre, float depth_thre, int32_t* idx_out, int32_t* cell_counts,
                      int32_t* status, void* stream);
+/* local_bestN, score_method 'flow_ratio' (kp_selection.py:135-160,192-199): ratio_out [H,W] fp32 = flow_diff / ||flow_fwd||, the
+ * norm sqrt(fx*fx + fy*fy) rounded step by step like NumPy's float32 np.linalg.norm, so ratio_out is bit-equal to the
+ * reference's fb_flow_mask (0/0 = NaN, x/0 = inf; neither passes `< thre`).  The cells select on the ratio with the depth mask as
+ * in dfvo_local_bestn; status[2] counts the RAW flow_diff < thre (the "case 1" early-out, kp_selection.py:121-125).  Outputs as
+ * dfvo_local_bestn. */
+int dfvo_local_bestn_flow_ratio(const float* flow_diff, const float* flow_fwd, const float* depth_diff, int H, int W, int rows,
+                                int cols, int num_bestN, float thre, float depth_thre, float* ratio_out, int32_t* idx_out,
+                                int32_t* cell_counts, int32_t* status, void* stream);
 /* bestN_flow_kp (kp_selection.py:33-71): N smallest of the whole map, ascending linear index. */
 size_t dfvo_bestn_workspace_bytes(int H, int W);
 int dfvo_bestn(const float* flow_diff, int H, int W, int N, int32_t* idx_out, void* workspace,
                size_t workspace_bytes, void* stream);
 /* kp1 = (x,y), kp2 = kp1 + flow_fwd[:,y,x] as float64 [n,2] (keypoint_sampler.py:101-104); compacts the
- * slots of dfvo_local_bestn (cell_counts != NULL) or takes all ncells*quota entries (bestN: ncells=1). */
+ * slots of dfvo_local_bestn (cell_counts != NULL) or takes all ncells*quota entries (bestN: ncells=1).  Also serves
+ * sampled_kp (kp_selection.py:327-378): idx = the constant uniform list of generate_kp_samples (keypoint_sampler.py:52-74) as
+ * full-image linear indices, cell_counts NULL, ncells 1. */
 int dfvo_gather_keypoints(const int32_t* idx, const int32_t* cell_counts, int ncells, int quota,
                           const float* flow_fwd, int H, int W, double* kp1, double* kp2, int32_t* n_out,
                           void* stream);

@@ -1,6 +1,8 @@
-"""Throughput of FramePipeline under the three tracking configurations the device runs: hybrid with GRIC model selection (the
-default), hybrid with the flow-magnitude check (ablation_model_sel_flow.yml: e_tracker.validity.method flow, thre 5) and PnP-only
-(ablation_tracker_pnp.yml: tracking_method PnP).  Same frames, analytic flow / depth injection and default execution mode as
+"""Throughput of FramePipeline under the tracking configurations the device runs: hybrid with GRIC model selection (the
+default), hybrid with the flow-magnitude check (ablation_model_sel_flow.yml: e_tracker.validity.method flow, thre 5), PnP-only
+(ablation_tracker_pnp.yml: tracking_method PnP), and the correspondence-selection ablations: uniformly sampled keypoints
+(ablation_correspondences_uniform.yml), global best-N (ablation_correspondences_best_n.yml) and local best-N with
+score_method flow_ratio.  Same frames, analytic flow / depth injection and default execution mode as
 bench.py (376x1241, three network engines in flight, pipelined tracker).  Prints one JSON line per configuration: frames/s and
 the tracker's host milliseconds per frame (enqueue + read, including its device waits) by branch.
 
@@ -20,7 +22,23 @@ import numpy as np  # noqa: E402
 
 import bench  # noqa: E402  (frame cycle and sizes only)
 
-CONFIGS = {"hybrid/GRIC": {}, "hybrid/flow": {"validity": dict(method="flow", thre=5)}, "PnP": {"tracking_method": "PnP"}}
+CONFIGS = {"hybrid/GRIC": {}, "hybrid/flow": {"e_tracker.validity": dict(method="flow", thre=5)}, "PnP": {"tracking_method": "PnP"},
+           "uniform": {"kp_selection.local_bestN.enable": False, "kp_selection.sampled_kp.enable": True, "e_tracker.kp_src": "kp_list",
+                       "scale_recovery.kp_src": "kp_list", "pnp_tracker.kp_src": "kp_list"},
+           "bestN": {"kp_selection.local_bestN.enable": False, "kp_selection.bestN.enable": True},
+           "local_bestN/flow_ratio": {"kp_selection.local_bestN.score_method": "flow_ratio"}}
+
+
+def configure(cfg, over):
+    """Sets the dotted keys of `over` in `cfg` (dict values become config nodes)."""
+    from b200 import config
+    for k, v in over.items():
+        node = cfg
+        *path, last = k.split(".")
+        for part in path:
+            node = node[part]
+        node[last] = config.AttrDict(v) if isinstance(v, dict) else v
+    return cfg
 
 
 def main():
@@ -53,11 +71,7 @@ def main():
             pipe.eng.depth_post(tmp, pipe.cfg.crop.depth_crop, 0.0, 50.0, st.raw_depth, st.depth)
 
     for name, over in CONFIGS.items():
-        cfg = config.default_cfg(H, W)
-        if "validity" in over:
-            cfg.e_tracker.validity = config.AttrDict(over["validity"])
-        if "tracking_method" in over:
-            cfg.tracking_method = over["tracking_method"]
+        cfg = configure(config.default_cfg(H, W), over)
         np.random.seed(4869)
         p = pipeline.FramePipeline(K, H, W, cfg=cfg, precision=native.PREC_BF16, runtime=rt, overlap=True, inflight=3, inject=inject,
                                    pipelined=True)
